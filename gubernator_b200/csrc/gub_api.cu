@@ -1216,6 +1216,9 @@ struct gub_p2p {
     uint32_t* counts = nullptr;    // [MAX_SHARDS]
     uint32_t* perm = nullptr;      // [cap]
     uint8_t* true_owner = nullptr; // [cap] (GLOBAL mode)
+    gub_req* expanded = nullptr;   // [cap] (GLOBAL mode) key-string steps: the expanded records, read by the hits queue
+    gub_params* params = nullptr;  // key-string steps with more than INLINE_PARAMS parameter sets: the table, grown on demand
+    size_t params_cap = 0;
     cudaEvent_t routed = nullptr;     // this parity's routing has been issued (ingest stream)
     cudaEvent_t step_done = nullptr;  // this parity's collect has completed (evaluation stream)
     bool step_done_valid = false;
@@ -1270,7 +1273,7 @@ void gub_p2p_destroy(gub_p2p* p) {
   if (p->s_eval) cudaStreamDestroy(p->s_eval);
   if (p->s_collect) cudaStreamDestroy(p->s_collect);
   for (auto& r : p->rt) {
-    void* rp[] = {r.tile_agg, r.counts, r.perm, r.true_owner};
+    void* rp[] = {r.tile_agg, r.counts, r.perm, r.true_owner, r.expanded, r.params};
     for (void* q : rp) if (q) cudaFree(q);
     if (r.routed) cudaEventDestroy(r.routed);
     if (r.step_done) cudaEventDestroy(r.step_done);
@@ -1416,6 +1419,46 @@ int p2p_route(gub_p2p* p, gub_p2p::Route* rt, const gub::P2PArgs& A, const gub_r
   return 0;
 }
 
+// What phase 1 of a step routes: 64-byte records, or a packed key-string batch (gub_keys_layout) with its parameter table (host memory).
+struct Ingest {
+  bool keys = false;
+  const gub_req* reqs = nullptr;
+  const uint8_t* packed = nullptr;
+  size_t packed_bytes = 0;
+  const gub_params* params = nullptr;
+  size_t n_params = 0;
+  int64_t created_base = 0;
+};
+
+// p2p_route for a key-string batch: one launch of k_p2p_route_keys.  A parameter table of more than INLINE_PARAMS sets is copied
+// on the ingest stream into this parity's table buffer (grown by p2p_phase_route).  GLOBAL mode: the expanded records also go to
+// this parity's scratch for the hits queue.
+int p2p_route_keys(gub_p2p* p, gub_p2p::Route* rt, const gub::P2PArgs& A, const Ingest& in, uint32_t n, int self_global, cudaStream_t si) {
+  gub_table* t = p->t;
+  gub::KeysRouteArgs K;
+  std::memset(&K, 0, sizeof K);
+  gub::RouteArgs& R = K.R;
+  R.P = A; R.reqs = nullptr; R.n = n; R.n_dev = nullptr; R.pts = t->d_ring_pts; R.pt_peer = t->d_ring_peers; R.lut = t->d_ring_lut; R.npts = t->ring_npts;
+  R.self_global = self_global; R.true_owner = self_global >= 0 ? rt->true_owner : nullptr; R.tile_agg = rt->tile_agg; R.counts = rt->counts; R.perm = rt->perm;
+  R.ticket = p->ticket;
+  const size_t bytes_at = (size_t)n * sizeof(gub_kreq) + ((size_t)n + 1) * 4;
+  K.packed = in.packed;
+  K.key_bytes = n ? in.packed_bytes - bytes_at : 0;
+  K.n_params = (uint32_t)in.n_params;
+  K.created_base = in.created_base;
+  K.expanded = self_global >= 0 ? rt->expanded : nullptr;
+  if (in.n_params <= gub::INLINE_PARAMS) {
+    if (in.n_params) std::memcpy(&K.Pi, in.params, in.n_params * sizeof(gub_params));
+  } else {
+    CK(cudaMemcpyAsync(rt->params, in.params, in.n_params * sizeof(gub_params), cudaMemcpyHostToDevice, si));
+    K.params_far = rt->params;
+  }
+  const uint32_t tiles = std::max<uint32_t>(1u, (n + gub::RT_THREADS - 1) / gub::RT_THREADS);
+  gub::k_p2p_route_keys<<<tiles, gub::RT_THREADS, 0, si>>>(K);
+  CK(cudaGetLastError());
+  return 0;
+}
+
 // The owner side of a step.  Default: the four-kernel pipeline reading the mailbox segments in place — k_seg_wait (one warp waits
 // for the sources' flags and writes the segment offsets), the batch kernels in ring mode (responses stored straight into the
 // sources' response mailboxes), k_seg_publish (response flags).  GUB_PATH=fused: one launch of the persistent kernel instead.
@@ -1470,30 +1513,53 @@ extern "C" {
 
 namespace {
 
-int p2p_step_check(gub_p2p* p, const gub_req* d_reqs, size_t n, const gub_clock* clk, gub_resp* d_out) {
-  if (!p || !clk || (n && (!d_reqs || !d_out))) return fail("gub_p2p_step: null argument");
-  if (n > p->cap) return fail("gub_p2p_step: n exceeds the mailbox capacity");
-  if (p->t->ring_cached != p->ring || p->t->ring_version != gub_ring_version_(p->ring)) return fail("gub_p2p_step: the table's ring changed since gub_p2p_create");
+int p2p_step_check(gub_p2p* p, const void* d_in, size_t n, const gub_clock* clk, gub_resp* d_out, const char* what = "gub_p2p_step") {
+  if (!p || !clk || (n && (!d_in || !d_out))) return fail(std::string(what) + ": null argument");
+  if (n > p->cap) return fail(std::string(what) + ": n exceeds the mailbox capacity");
+  if (p->t->ring_cached != p->ring || p->t->ring_version != gub_ring_version_(p->ring)) return fail(std::string(what) + ": the table's ring changed since gub_p2p_create");
+  return 0;
+}
+
+// The checks of p2p_step_check plus those of a key-string batch (the offsets themselves are device memory: the kernel clamps them).
+int p2p_step_keys_check(gub_p2p* p, const void* d_packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params, const gub_clock* clk,
+                        gub_resp* d_out, const char* what) {
+  if (p2p_step_check(p, d_packed, n, clk, d_out, what)) return -1;
+  if (n_params && !params) return fail(std::string(what) + ": null argument");
+  if (n_params > 0xFFFFFFFFull) return fail(std::string(what) + ": too many parameter sets");
+  if (n && packed_bytes < n * sizeof(gub_kreq) + (n + 1) * 4) return fail(std::string(what) + ": packed buffer smaller than its records and offsets");
   return 0;
 }
 
 // Phase 1 of a step, on the ingest stream: partition by owner and store the records into the owners' mailboxes.  This parity's
 // scratch and mailbox halves were last used two steps ago; that step's collect (on the evaluation stream) must have finished,
 // which also means every peer has drained what we sent it then.
-int p2p_phase_route(gub_p2p* p, const gub_req* d_reqs, size_t n, cudaStream_t si, cudaStream_t st) {
+int p2p_phase_route(gub_p2p* p, const Ingest& in, size_t n, cudaStream_t si, cudaStream_t st) {
   gub_table* t = p->t;
   std::lock_guard<std::mutex> lk(t->mu);
   CK(cudaSetDevice(t->device));
   const bool two = si != st;
+  if (in.keys && in.n_params > gub::INLINE_PARAMS) {  // grow the next parity's parameter table before the step counts as started
+    gub_p2p::Route* nx = &p->rt[(p->epoch + 1) & 1u];
+    if (nx->params_cap < in.n_params) {
+      if (nx->params) CK(cudaFree(nx->params));
+      nx->params = nullptr; nx->params_cap = 0;
+      CK(cudaMalloc(&nx->params, in.n_params * sizeof(gub_params)));
+      nx->params_cap = in.n_params;
+    }
+  }
   p->epoch++;
   gub_p2p::Route* rt = &p->rt[p->epoch & 1u];
   gub::P2PArgs A;
   p2p_args(p, A);
   if (two && rt->step_done_valid) CK(cudaStreamWaitEvent(si, rt->step_done, 0));
   const int self_global = p->hits_q ? (int)p->rank : -1;
-  if (p2p_route(p, rt, A, d_reqs, (uint32_t)n, nullptr, self_global, si)) return -1;
+  if (in.keys) {
+    if (p2p_route_keys(p, rt, A, in, (uint32_t)n, self_global, si)) return -1;
+  } else {
+    if (p2p_route(p, rt, A, in.reqs, (uint32_t)n, nullptr, self_global, si)) return -1;
+  }
   if (p->hits_q && n) {  // a non-owner queues the hits of its GLOBAL requests (gubernator.go:402-404, global.go:74-78)
-    if (gq_accumulate(p->hits_q, d_reqs, n, nullptr, rt->true_owner, p->rank, p->seq, si)) return -1;
+    if (gq_accumulate(p->hits_q, in.keys ? rt->expanded : in.reqs, n, nullptr, rt->true_owner, p->rank, p->seq, si)) return -1;
   }
   if (two) CK(cudaEventRecord(rt->routed, si));
   return 0;
@@ -1533,31 +1599,43 @@ int p2p_phase_collect(gub_p2p* p, size_t n, gub_resp* d_out, cudaStream_t si, cu
   return 0;
 }
 
+int p2p_step_streams(gub_p2p* p, const Ingest& in, size_t n, const gub_clock* clk, gub_resp* d_out, void* ingest_stream, void* stream);
+
 }  // namespace
 
 extern "C" {
 
 int gub_p2p_step_streams(gub_p2p* p, const gub_req* d_reqs, size_t n, const gub_clock* clk, gub_resp* d_out, void* ingest_stream, void* stream) {
   if (p2p_step_check(p, d_reqs, n, clk, d_out)) return -1;
+  Ingest in;
+  in.reqs = d_reqs;
+  return p2p_step_streams(p, in, n, clk, d_out, ingest_stream, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+int p2p_step_streams(gub_p2p* p, const Ingest& in, size_t n, const gub_clock* clk, gub_resp* d_out, void* ingest_stream, void* stream) {
   cudaStream_t st = (cudaStream_t)stream, si = (cudaStream_t)ingest_stream;
   // Default: routing on the ingest stream, evaluation and collect on `stream`.  GUB_RING_STREAMS=3 (experimental) moves the evaluation
   // and the collect — which waits for the slowest owner — onto streams of the ring's own, so that step e+1 is evaluated while step e's
   // answers travel; that variant has been seen to stall under the per-kernel profiling events.
   static const int own_streams = [] { const char* e = getenv("GUB_RING_STREAMS"); return e ? std::atoi(e) : 2; }();
   if (si != st && own_streams < 3) {
-    if (p2p_phase_route(p, d_reqs, n, si, st)) return -1;
+    if (p2p_phase_route(p, in, n, si, st)) return -1;
     if (p2p_phase_evaluate(p, clk, st)) return -1;
     return p2p_phase_collect(p, n, d_out, si, st);
   }
   if (si == st) {  // one stream: the three phases in stream order
-    if (p2p_phase_route(p, d_reqs, n, si, st)) return -1;
+    if (p2p_phase_route(p, in, n, si, st)) return -1;
     if (p2p_phase_evaluate(p, clk, st)) return -1;
     return p2p_phase_collect(p, n, d_out, si, st);
   }
   // Two caller streams: routing on the ingest stream; the owner-side evaluation on our own evaluation stream (it synchronises with
   // the peers through the mailbox flags, not through the caller's streams); the collect — which waits for the slowest owner — on our
   // collect stream; `stream` then waits for the collect only.  Step e+1 is routed and evaluated while step e's answers travel.
-  if (p2p_phase_route(p, d_reqs, n, si, p->s_collect)) return -1;
+  if (p2p_phase_route(p, in, n, si, p->s_collect)) return -1;
   if (p2p_phase_evaluate(p, clk, p->s_eval)) return -1;
   CK(cudaEventRecord(p->ev_fork, st));                 // d_out is ours to write once everything queued on `stream` so far is done
   CK(cudaStreamWaitEvent(p->s_collect, p->ev_fork, 0));
@@ -1565,6 +1643,25 @@ int gub_p2p_step_streams(gub_p2p* p, const gub_req* d_reqs, size_t n, const gub_
   CK(cudaStreamWaitEvent(st, p->rt[p->epoch & 1u].step_done, 0));
   p->last_ingest = si; p->own_streams_used = true;
   return 0;
+}
+
+Ingest keys_ingest(const void* d_packed, size_t packed_bytes, const gub_params* params, size_t n_params, int64_t created_base) {
+  Ingest in;
+  in.keys = true; in.packed = static_cast<const uint8_t*>(d_packed); in.packed_bytes = packed_bytes;
+  in.params = params; in.n_params = n_params; in.created_base = created_base;
+  return in;
+}
+
+}  // namespace
+
+extern "C" {
+
+/* Key strings in (gub_keys_layout, on the shard's device), responses out: k_p2p_route_keys hashes, expands and routes in one launch,
+ * then the step goes on exactly as gub_p2p_step_streams. */
+int gub_p2p_step_keys(gub_p2p* p, const void* d_packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params, int64_t created_base,
+                      const gub_clock* clk, gub_resp* d_out, void* ingest_stream, void* stream) {
+  if (p2p_step_keys_check(p, d_packed, packed_bytes, n, params, n_params, clk, d_out, "gub_p2p_step_keys")) return -1;
+  return p2p_step_streams(p, keys_ingest(d_packed, packed_bytes, params, n_params, created_base), n, clk, d_out, ingest_stream, stream);
 }
 
 }  // extern "C"
@@ -1586,6 +1683,17 @@ int local_phase_sync(gub_p2p* const* ps, uint32_t world, void* const* streams) {
   }
   return 0;
 }
+
+// The phases of every shard in order: all routings, then all evaluations, then all collects (arguments checked by the caller).
+int p2p_local_all(gub_p2p* const* ps, uint32_t world, const Ingest* in, const size_t* n, const gub_clock* clk, gub_resp* const* d_out,
+                  void* const* streams) {
+  for (uint32_t r = 0; r < world; r++) if (p2p_phase_route(ps[r], in[r], n[r], (cudaStream_t)streams[r], (cudaStream_t)streams[r])) return -1;
+  if (local_phase_sync(ps, world, streams)) return -1;
+  for (uint32_t r = 0; r < world; r++) if (p2p_phase_evaluate(ps[r], clk, (cudaStream_t)streams[r])) return -1;
+  if (local_phase_sync(ps, world, streams)) return -1;
+  for (uint32_t r = 0; r < world; r++) if (p2p_phase_collect(ps[r], n[r], d_out[r], (cudaStream_t)streams[r], (cudaStream_t)streams[r])) return -1;
+  return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -1597,12 +1705,36 @@ int gub_p2p_step_local_all(gub_p2p* const* ps, uint32_t world, const gub_req* co
                            gub_resp* const* d_out, void* const* streams) {
   if (!ps || !d_reqs || !n || !d_out || !streams || world == 0) return fail("gub_p2p_step_local_all: bad argument");
   for (uint32_t r = 0; r < world; r++) if (p2p_step_check(ps[r], d_reqs[r], n[r], clk, d_out[r])) return -1;
-  for (uint32_t r = 0; r < world; r++) if (p2p_phase_route(ps[r], d_reqs[r], n[r], (cudaStream_t)streams[r], (cudaStream_t)streams[r])) return -1;
-  if (local_phase_sync(ps, world, streams)) return -1;
-  for (uint32_t r = 0; r < world; r++) if (p2p_phase_evaluate(ps[r], clk, (cudaStream_t)streams[r])) return -1;
-  if (local_phase_sync(ps, world, streams)) return -1;
-  for (uint32_t r = 0; r < world; r++) if (p2p_phase_collect(ps[r], n[r], d_out[r], (cudaStream_t)streams[r], (cudaStream_t)streams[r])) return -1;
-  return 0;
+  std::vector<Ingest> in(world);
+  for (uint32_t r = 0; r < world; r++) in[r].reqs = d_reqs[r];
+  return p2p_local_all(ps, world, in.data(), n, clk, d_out, streams);
+}
+
+/* gub_p2p_step_local_all with key strings: shard r ingests the packed batch d_packed[r] (n[r] requests, on its device); one parameter
+ * table for all shards. */
+int gub_p2p_step_keys_local_all(gub_p2p* const* ps, uint32_t world, const void* const* d_packed, const size_t* packed_bytes, const size_t* n,
+                                const gub_params* params, size_t n_params, int64_t created_base, const gub_clock* clk, gub_resp* const* d_out,
+                                void* const* streams) {
+  return gub_p2p_step_mixed_local_all(ps, world, nullptr, d_packed, packed_bytes, n, params, n_params, created_base, clk, d_out, streams);
+}
+
+/* Both kinds of ingest in one step: shard r ingests key strings when d_packed[r] != NULL, else the records d_reqs[r]. */
+int gub_p2p_step_mixed_local_all(gub_p2p* const* ps, uint32_t world, const gub_req* const* d_reqs, const void* const* d_packed, const size_t* packed_bytes,
+                                 const size_t* n, const gub_params* params, size_t n_params, int64_t created_base, const gub_clock* clk,
+                                 gub_resp* const* d_out, void* const* streams) {
+  const char* what = d_reqs ? "gub_p2p_step_mixed_local_all" : "gub_p2p_step_keys_local_all";
+  if (!ps || !d_packed || !packed_bytes || !n || !d_out || !streams || world == 0) return fail(std::string(what) + ": bad argument");
+  std::vector<Ingest> in(world);
+  for (uint32_t r = 0; r < world; r++) {
+    if (d_packed[r] || !d_reqs) {
+      if (p2p_step_keys_check(ps[r], d_packed[r], packed_bytes[r], n[r], params, n_params, clk, d_out[r], what)) return -1;
+      in[r] = keys_ingest(d_packed[r], packed_bytes[r], params, n_params, created_base);
+    } else {
+      if (p2p_step_check(ps[r], d_reqs[r], n[r], clk, d_out[r], what)) return -1;
+      in[r].reqs = d_reqs[r];
+    }
+  }
+  return p2p_local_all(ps, world, in.data(), n, clk, d_out, streams);
 }
 
 int gub_p2p_step(gub_p2p* p, const gub_req* d_reqs, size_t n, const gub_clock* clk, gub_resp* d_out, void* stream) {
@@ -1739,6 +1871,7 @@ int gub_p2p_enable_global(gub_p2p* p, uint32_t capacity) {
   CK(cudaMalloc(&p->g_count, 16));
   CK(cudaMemset(p->g_count, 0, 16));
   CK(cudaMalloc(&p->g_counts_all, gub::MAX_SHARDS * 4));
+  for (auto& r : p->rt) CK(cudaMalloc(&r.expanded, (size_t)p->cap * sizeof(gub_req)));
   CK(cudaHostAlloc(&p->h_counts, 16, cudaHostAllocDefault));
   std::memset(p->h_counts, 0, 16);
   if (gq_reserve(p->updates_q, (size_t)p->world * p->cap, 0)) return -1;

@@ -1137,15 +1137,19 @@ __global__ void __launch_bounds__(256) k_hash_keys(const uint8_t* bytes, const u
 }
 
 // ---- compact requests -> gub_req records (see gub_creq in the header) --------------------------------------------------
-__device__ __forceinline__ void expand_one(const gub_creq* creqs, uint32_t i, ulonglong2 q0, ulonglong2 q1, bool known, ulonglong2 a, ulonglong2 b,
-                                           int64_t created_base, gub_req* out) {
+__device__ __forceinline__ void expand_words(ulonglong2 q0, ulonglong2 q1, bool known, ulonglong2 a, ulonglong2 b, int64_t created_base,
+                                             ulonglong2& w0, ulonglong2& w1, ulonglong2& w2, ulonglong2& w3) {
   if (!known) { q0 = make_ulonglong2(0, 0); q1 = make_ulonglong2(0, 0xFFFFFFFFull); }  // unknown parameter set -> invalid algorithm (in-band error)
   const int32_t delta = (int32_t)(uint32_t)(b.y >> 32);
+  w0 = a;                                                                   // key_xxh64, key_fnv1
+  w1 = make_ulonglong2(b.x, q0.x);                                          // hits, limit
+  w2 = make_ulonglong2(q0.y, q1.x);                                         // duration, burst
+  w3 = make_ulonglong2((uint64_t)wadd(created_base, (int64_t)delta), q1.y); // created_at, algorithm | behavior << 32
+}
+__device__ __forceinline__ void expand_one(const gub_creq* creqs, uint32_t i, ulonglong2 q0, ulonglong2 q1, bool known, ulonglong2 a, ulonglong2 b,
+                                           int64_t created_base, gub_req* out) {
   ulonglong2* o = reinterpret_cast<ulonglong2*>(out + i);
-  o[0] = a;                                                                   // key_xxh64, key_fnv1
-  o[1] = make_ulonglong2(b.x, q0.x);                                          // hits, limit
-  o[2] = make_ulonglong2(q0.y, q1.x);                                         // duration, burst
-  o[3] = make_ulonglong2((uint64_t)wadd(created_base, (int64_t)delta), q1.y); // created_at, algorithm | behavior << 32
+  expand_words(q0, q1, known, a, b, created_base, o[0], o[1], o[2], o[3]);
 }
 
 __global__ void __launch_bounds__(256) k_expand(const gub_creq* creqs, uint32_t n, const gub_params* params, uint32_t n_params, int64_t created_base,
@@ -1184,6 +1188,23 @@ __global__ void __launch_bounds__(256) k_expand_inline(const gub_creq* creqs, ui
 // ---- key strings -> gub_req records: HashKey (client.go:39-41) + XXH64 (workers.go:153) + FNV-1 (replicated_hash.go:108) on the
 // device, fused with the expansion of the per-limit parameters.  One packed buffer per batch: [gub_kreq x n][uint32 offsets x (n+1)]
 // [key bytes], key i = bytes[offsets[i] .. offsets[i+1]).
+// kreq_decode: one request of such a batch -> its gub_req record as four 16-byte words (the layout of expand_one).  kr = the request's
+// gub_kreq (hits | params, created_delta); key = its len key bytes; params_far != nullptr: the table lives in device memory, else in P.
+__device__ __forceinline__ void kreq_decode(const ulonglong2 kr, const uint8_t* key, uint32_t len, const InlineParams& P, uint32_t n_params,
+                                            const gub_params* params_far, int64_t created_base, ulonglong2& w0, ulonglong2& w1, ulonglong2& w2,
+                                            ulonglong2& w3) {
+  uint64_t xxh, fnv;
+  hash_key_bytes(key, len, &xxh, &fnv);
+  const uint32_t pi = (uint32_t)(kr.y & 0xFFFFFFFFull);
+  const bool known = pi < n_params;
+  ulonglong2 q0 = make_ulonglong2(0, 0), q1 = q0;
+  if (known) {
+    if (params_far) { const ulonglong2* pp = reinterpret_cast<const ulonglong2*>(params_far + pi); q0 = __ldg(pp); q1 = __ldg(pp + 1); }
+    else { q0 = P.q[pi][0]; q1 = P.q[pi][1]; }
+  }
+  expand_words(q0, q1, known, make_ulonglong2(xxh, fnv), kr, created_base, w0, w1, w2, w3);
+}
+
 __global__ void __launch_bounds__(256) k_hash_expand(const uint8_t* packed, uint32_t n, const InlineParams P, uint32_t n_params, const gub_params* params_far,
                                                      int64_t created_base, gub_req* out) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1192,16 +1213,8 @@ __global__ void __launch_bounds__(256) k_hash_expand(const uint8_t* packed, uint
   const uint32_t* offsets = reinterpret_cast<const uint32_t*>(packed + (size_t)n * 16);
   const uint8_t* bytes = packed + (size_t)n * 16 + ((size_t)n + 1) * 4;
   const uint32_t lo = __ldg(offsets + i), hi = __ldg(offsets + i + 1);
-  uint64_t xxh, fnv;
-  hash_key_bytes(bytes + lo, hi - lo, &xxh, &fnv);
-  const uint32_t pi = (uint32_t)(kr.y & 0xFFFFFFFFull);
-  const bool known = pi < n_params;
-  ulonglong2 q0 = make_ulonglong2(0, 0), q1 = q0;
-  if (known) {
-    if (params_far) { const ulonglong2* pp = reinterpret_cast<const ulonglong2*>(params_far + pi); q0 = __ldg(pp); q1 = __ldg(pp + 1); }
-    else { q0 = P.q[pi][0]; q1 = P.q[pi][1]; }
-  }
-  expand_one(nullptr, i, q0, q1, known, make_ulonglong2(xxh, fnv), kr, created_base, out);
+  ulonglong2* o = reinterpret_cast<ulonglong2*>(out + i);
+  kreq_decode(kr, bytes + lo, hi - lo, P, n_params, params_far, created_base, o[0], o[1], o[2], o[3]);
 }
 
 // ---- maintenance kernels -------------------------------------------------------------------------------------

@@ -83,42 +83,50 @@ __device__ __forceinline__ uint32_t ring_owner_lut(const RouteArgs& R, uint64_t 
   return (uint32_t)__ldg(R.pt_peer + idx);
 }
 
-__global__ void __launch_bounds__(RT_THREADS) k_p2p_route(const RouteArgs R) {
-  __shared__ uint32_t s_tile, s_last;
-  __shared__ uint32_t s_cnt[MAX_SHARDS], s_off[MAX_SHARDS];
-  __shared__ uint16_t s_w[MAX_SHARDS][RT_WARPS];
+// The parts of a routing CTA that do not depend on where its records come from (k_p2p_route: 64-byte records; k_p2p_route_keys:
+// key strings hashed and expanded on the spot).
+struct RouteSmem {
+  uint32_t tile, last;
+  uint32_t cnt[MAX_SHARDS], off[MAX_SHARDS];
+  uint16_t w[MAX_SHARDS][RT_WARPS];
+};
+
+// Takes the CTA's tile ticket and clears the per-owner counts; returns the tile.
+__device__ __forceinline__ uint32_t route_tile_begin(const RouteArgs& R, RouteSmem& S) {
+  const uint32_t tid = threadIdx.x;
+  if (tid == 0) S.tile = atomicAdd(&R.ticket[0], 1u);
+  if (tid < MAX_SHARDS) S.cnt[tid] = 0;
+  for (uint32_t k = tid; k < (uint32_t)(MAX_SHARDS * RT_WARPS); k += RT_THREADS) (&S.w[0][0])[k] = 0;
+  __syncthreads();
+  return S.tile;
+}
+
+// Owner of request i by its FNV-1 hash (replicated_hash.go:104-119), recorded for the GLOBAL hits queue; a GLOBAL request this shard
+// does not own is rewritten in r3 and stays here.
+__device__ __forceinline__ uint32_t route_owner(const RouteArgs& R, uint32_t i, uint64_t fnv, ulonglong2& r3) {
+  uint32_t o = ring_owner_lut(R, fnv);
+  if (R.true_owner) R.true_owner[i] = (uint8_t)o;
+  if (R.self_global >= 0 && o != (uint32_t)R.self_global && ((uint32_t)(r3.y >> 32) & GUB_BEHAVIOR_GLOBAL)) {
+    // GLOBAL on a non-owner: answered here from the replica, as a clone with NO_BATCHING set, GLOBAL cleared, IsOwner = false (gubernator.go:408-411)
+    o = (uint32_t)R.self_global;
+    uint32_t beh = (uint32_t)(r3.y >> 32);
+    beh = (beh | (uint32_t)GUB_BEHAVIOR_NO_BATCHING) & ~(uint32_t)(GUB_BEHAVIOR_GLOBAL | GUB_REQ_IS_OWNER);
+    r3.y = (r3.y & 0xFFFFFFFFull) | ((unsigned long long)beh << 32);
+  }
+  return o;
+}
+
+// Stable partition of the tile by owner (per-warp counts per owner give the rank inside the tile), tile publication, NVLink stores
+// into the owners' mailboxes, perm, and — in the last tile to finish — the totals and the epoch-tagged flag release.
+__device__ __forceinline__ void route_tile_end(const RouteArgs& R, RouteSmem& S, uint32_t t, uint32_t ntiles, uint32_t i, bool valid, uint32_t o,
+                                               const ulonglong2& r0, const ulonglong2& r1, const ulonglong2& r2, const ulonglong2& r3) {
   const P2PArgs& P = R.P;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) s_tile = atomicAdd(&R.ticket[0], 1u);
-  if (tid < MAX_SHARDS) s_cnt[tid] = 0;
-  for (uint32_t k = tid; k < (uint32_t)(MAX_SHARDS * RT_WARPS); k += RT_THREADS) (&s_w[0][0])[k] = 0;
-  __syncthreads();
-  const uint32_t t = s_tile;
-  const uint32_t n = R.n_dev ? min(__ldcg(R.n_dev), R.n) : R.n;
-  const uint32_t ntiles = (n + RT_THREADS - 1) / RT_THREADS;
-  const uint32_t i = t * RT_THREADS + tid;
-  const bool valid = i < n;
-  // owner of my request; per-warp counts per owner give the stable rank inside the tile
-  uint32_t o = 0xFFu;
-  ulonglong2 r0, r1, r2, r3;
-  if (valid) {
-    const ulonglong2* src = reinterpret_cast<const ulonglong2*>(R.reqs + i);
-    r0 = __ldg(src); r1 = __ldg(src + 1); r2 = __ldg(src + 2); r3 = __ldg(src + 3);
-    o = ring_owner_lut(R, r0.y);
-    if (R.true_owner) R.true_owner[i] = (uint8_t)o;
-    if (R.self_global >= 0 && o != (uint32_t)R.self_global && ((uint32_t)(r3.y >> 32) & GUB_BEHAVIOR_GLOBAL)) {
-      // GLOBAL on a non-owner: answered here from the replica, as a clone with NO_BATCHING set, GLOBAL cleared, IsOwner = false (gubernator.go:408-411)
-      o = (uint32_t)R.self_global;
-      uint32_t beh = (uint32_t)(r3.y >> 32);
-      beh = (beh | (uint32_t)GUB_BEHAVIOR_NO_BATCHING) & ~(uint32_t)(GUB_BEHAVIOR_GLOBAL | GUB_REQ_IS_OWNER);
-      r3.y = (r3.y & 0xFFFFFFFFull) | ((unsigned long long)beh << 32);
-    }
-  }
   const uint32_t mates = __match_any_sync(0xFFFFFFFFu, valid ? o : (0x100u | lane));
-  if (valid && lane == (uint32_t)(__ffs(mates) - 1)) { s_w[o][warp] = (uint16_t)__popc(mates); atomicAdd(&s_cnt[o], (uint32_t)__popc(mates)); }
+  if (valid && lane == (uint32_t)(__ffs(mates) - 1)) { S.w[o][warp] = (uint16_t)__popc(mates); atomicAdd(&S.cnt[o], (uint32_t)__popc(mates)); }
   __syncthreads();
   // publish this tile's counts, then sum the tiles before it (warp o handles owner o)
-  if (t < ntiles && tid < P.world) __stcg(&R.tile_agg[(size_t)t * MAX_SHARDS + tid], ((unsigned long long)P.epoch << 32) | (unsigned long long)s_cnt[tid]);
+  if (t < ntiles && tid < P.world) __stcg(&R.tile_agg[(size_t)t * MAX_SHARDS + tid], ((unsigned long long)P.epoch << 32) | (unsigned long long)S.cnt[tid]);
   if (warp < P.world && t < ntiles) {
     uint32_t sum = 0;
     for (uint32_t tp = lane; tp < t; tp += 32) {
@@ -129,32 +137,93 @@ __global__ void __launch_bounds__(RT_THREADS) k_p2p_route(const RouteArgs R) {
       sum += (uint32_t)(v & 0xFFFFFFFFull);
     }
     sum = __reduce_add_sync(0xFFFFFFFFu, sum);
-    if (lane == 0) s_off[warp] = sum;
+    if (lane == 0) S.off[warp] = sum;
   }
   __syncthreads();
   if (valid) {
     uint32_t before = 0;
 #pragma unroll
-    for (int w = 0; w < RT_WARPS; w++) before += ((uint32_t)w < warp) ? (uint32_t)s_w[o][w] : 0u;
-    const uint32_t pos = s_off[o] + before + __popc(mates & ((1u << lane) - 1u));  // position within (me -> owner o)'s mailbox segment
+    for (int w = 0; w < RT_WARPS; w++) before += ((uint32_t)w < warp) ? (uint32_t)S.w[o][w] : 0u;
+    const uint32_t pos = S.off[o] + before + __popc(mates & ((1u << lane) - 1u));  // position within (me -> owner o)'s mailbox segment
     ulonglong2* dst = reinterpret_cast<ulonglong2*>(P.peers[o].req_mb + mb_index(P, P.rank, pos));  // NVLink store
     dst[0] = r0; dst[1] = r1; dst[2] = r2; dst[3] = r3;
     // the way back: responses of owner o come back in its response mailbox at `pos`; (o, pos) packed for the un-route
     R.perm[i] = (o << 24) | pos;
   }
   // the last tile knows the totals
-  if (t + 1 == ntiles && tid < P.world) R.counts[tid] = s_off[tid] + s_cnt[tid];
+  if (t + 1 == ntiles && tid < P.world) R.counts[tid] = S.off[tid] + S.cnt[tid];
   if (ntiles == 0 && t == 0 && tid < P.world) R.counts[tid] = 0;
   __threadfence_system();
   __syncthreads();
-  if (tid == 0) s_last = atomicAdd(&R.ticket[1], 1u) == gridDim.x - 1 ? 1u : 0u;
+  if (tid == 0) S.last = atomicAdd(&R.ticket[1], 1u) == gridDim.x - 1 ? 1u : 0u;
   __syncthreads();
-  if (s_last) {  // every tile has been stored: tell every owner how many records it got from us
+  if (S.last) {  // every tile has been stored: tell every owner how many records it got from us
     __threadfence_system();
     if (tid < P.world)
       st_release_sys(&P.peers[tid].req_flag[(size_t)(P.epoch & 1u) * P.world + P.rank], ((unsigned long long)P.epoch << 32) | (unsigned long long)__ldcg(&R.counts[tid]));
     if (tid == 0) { R.ticket[0] = 0; R.ticket[1] = 0; }
   }
+}
+
+__global__ void __launch_bounds__(RT_THREADS) k_p2p_route(const RouteArgs R) {
+  __shared__ RouteSmem S;
+  const uint32_t t = route_tile_begin(R, S);
+  const uint32_t n = R.n_dev ? min(__ldcg(R.n_dev), R.n) : R.n;
+  const uint32_t ntiles = (n + RT_THREADS - 1) / RT_THREADS;
+  const uint32_t i = t * RT_THREADS + threadIdx.x;
+  const bool valid = i < n;
+  uint32_t o = 0xFFu;
+  ulonglong2 r0, r1, r2, r3;
+  if (valid) {
+    const ulonglong2* src = reinterpret_cast<const ulonglong2*>(R.reqs + i);
+    r0 = __ldg(src); r1 = __ldg(src + 1); r2 = __ldg(src + 2); r3 = __ldg(src + 3);
+    o = route_owner(R, i, r0.y, r3);
+  }
+  route_tile_end(R, S, t, ntiles, i, valid, o, r0, r1, r2, r3);
+}
+
+// ---- routing straight from key strings --------------------------------------------------------------------------------------
+// k_p2p_route_keys = k_hash_expand + k_p2p_route in one launch: every thread hashes its key (XXH64 + FNV-1), expands its parameter set
+// into the 64-byte record and routes it exactly like k_p2p_route (same owner lookup by FNV-1, same stable partition, same mailbox
+// layout), so that a step may mix shards that ingest key strings with shards that ingest records.  The packed buffer
+// ([gub_kreq x n][uint32 offsets x (n + 1)][key bytes], gub_keys_layout) is device memory the host cannot check, so the key bounds
+// are clamped here: hi = min(offsets[i + 1], key_bytes), lo = min(offsets[i], hi); a malformed entry is hashed as that (possibly
+// empty) key and nothing outside the buffer is read.  The host checks that the buffer holds the records and offsets.
+struct KeysRouteArgs {
+  RouteArgs R;                     // R.reqs is unused
+  const uint8_t* packed;
+  uint64_t key_bytes;              // bytes after the offsets (packed_bytes - bytes_at)
+  InlineParams Pi;                 // the parameter table when n_params <= INLINE_PARAMS ...
+  const gub_params* params_far;    // ... else here (device memory)
+  uint32_t n_params;
+  int64_t created_base;
+  gub_req* expanded;               // optional [n]: the expanded records by original index (input of the GLOBAL hits queue)
+};
+
+__global__ void __launch_bounds__(RT_THREADS) k_p2p_route_keys(const KeysRouteArgs K) {
+  __shared__ RouteSmem S;
+  const RouteArgs& R = K.R;
+  const uint32_t t = route_tile_begin(R, S);
+  const uint32_t n = R.n;
+  const uint32_t ntiles = (n + RT_THREADS - 1) / RT_THREADS;
+  const uint32_t i = t * RT_THREADS + threadIdx.x;
+  const bool valid = i < n;
+  uint32_t o = 0xFFu;
+  ulonglong2 r0, r1, r2, r3;
+  if (valid) {
+    const ulonglong2 kr = __ldcs(reinterpret_cast<const ulonglong2*>(K.packed) + i);  // hits | params, created_delta
+    const uint32_t* offsets = reinterpret_cast<const uint32_t*>(K.packed + (size_t)n * 16);
+    const uint8_t* bytes = K.packed + (size_t)n * 16 + ((size_t)n + 1) * 4;
+    const uint64_t hi = min((uint64_t)__ldg(offsets + i + 1), K.key_bytes);
+    const uint64_t lo = min((uint64_t)__ldg(offsets + i), hi);
+    kreq_decode(kr, bytes + lo, (uint32_t)(hi - lo), K.Pi, K.n_params, K.params_far, K.created_base, r0, r1, r2, r3);
+    if (K.expanded) {
+      ulonglong2* e = reinterpret_cast<ulonglong2*>(K.expanded + i);
+      e[0] = r0; e[1] = r1; e[2] = r2; e[3] = r3;
+    }
+    o = route_owner(R, i, r0.y, r3);
+  }
+  route_tile_end(R, S, t, ntiles, i, valid, o, r0, r1, r2, r3);
 }
 
 // Source side: wait for every owner's response flag, then out[i] = resp_mb[owner(i)][pos(i)] (perm as written by k_p2p_route).

@@ -36,7 +36,8 @@ EXPORTS = ["gub_create", "gub_destroy", "gub_last_error", "gub_abi_version", "gu
            "gub_gq_destroy", "gub_gq_accumulate_device", "gub_gq_drain_device", "gub_make_updates_device", "gub_add_items_device",
            "gub_route_owner_device", "gub_route_global_device", "gub_p2p_create", "gub_p2p_destroy", "gub_p2p_export", "gub_p2p_connect",
            "gub_p2p_connect_local", "gub_p2p_step", "gub_p2p_step_streams", "gub_p2p_status", "gub_p2p_enable_global", "gub_nccl_unique_id",
-           "gub_p2p_nccl_init", "gub_p2p_nccl_init_local", "gub_global_tick", "gub_gq_dropped", "gub_set_sweep", "gub_set_trace", "gub_get_trace", "gub_get_trace_raw", "gub_get_ktrace", "gub_keys_layout", "gub_submit_keys_async", "gub_global_tick_local_all", "gub_p2p_step_local_all"]
+           "gub_p2p_nccl_init", "gub_p2p_nccl_init_local", "gub_global_tick", "gub_gq_dropped", "gub_set_sweep", "gub_set_trace", "gub_get_trace", "gub_get_trace_raw", "gub_get_ktrace", "gub_keys_layout", "gub_submit_keys_async", "gub_global_tick_local_all", "gub_p2p_step_local_all",
+           "gub_p2p_step_keys", "gub_p2p_step_keys_local_all", "gub_p2p_step_mixed_local_all"]
 
 
 class Config(C.Structure):
@@ -127,6 +128,23 @@ def lib():
         L.gub_keys_layout.argtypes = [sz, sz, C.POINTER(sz), C.POINTER(sz), C.POINTER(sz)]
         _lib = L
     return _lib
+
+
+_vp, _sz, _pvp, _psz = C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p), C.POINTER(C.c_size_t)
+# The ring's key-string entries are bound when first called, so that a library built without them (the CPU emulation of the C ABI
+# that the host-layer tests load) still loads; calling one that a library lacks raises.
+_LATE_ARGTYPES = {
+    "gub_p2p_step_keys": [_vp, _vp, _sz, _sz, _vp, _sz, C.c_int64, _vp, _vp, _vp, _vp],
+    "gub_p2p_step_keys_local_all": [_pvp, C.c_uint32, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, _pvp, _pvp],
+    "gub_p2p_step_mixed_local_all": [_pvp, C.c_uint32, _pvp, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, _pvp, _pvp],
+}
+
+
+def _entry(name):
+    fn = getattr(lib(), name)
+    if fn.argtypes is None:
+        fn.argtypes = _LATE_ARGTYPES[name]
+    return fn
 
 
 def _check(rc, what):
@@ -394,6 +412,13 @@ class P2P:
         else:
             _check(lib().gub_p2p_step_streams(self._h, d_reqs_ptr, n, clk.ctypes.data, d_out_ptr, ingest_stream, stream), "gub_p2p_step_streams")
 
+    def step_keys(self, d_packed_ptr, packed_bytes, n, params, created_base, clk, d_out_ptr, stream=0, ingest_stream=None):
+        """One step fed with key strings (gub_p2p_step_keys): d_packed_ptr = a pack_keys() buffer on this shard's device, params = the
+        PARAMS_DTYPE table (host).  ingest_stream None: one stream for the whole step."""
+        params = _params_array(params)
+        _check(_entry("gub_p2p_step_keys")(self._h, d_packed_ptr, packed_bytes, n, params.ctypes.data if len(params) else None, len(params), int(created_base),
+                                       clk.ctypes.data, d_out_ptr, stream if ingest_stream is None else ingest_stream, stream), "gub_p2p_step_keys")
+
     def status(self):
         """Raises when a bounded device-side wait of an earlier step gave up (a shard of the ring is not answering)."""
         e = C.c_int(0)
@@ -454,6 +479,32 @@ def p2p_step_local_all(p2ps, req_ptrs, ns, clk, out_ptrs, streams):
     W = len(p2ps)
     _check(lib().gub_p2p_step_local_all((C.c_void_p * W)(*[p._h for p in p2ps]), W, (C.c_void_p * W)(*req_ptrs), (C.c_size_t * W)(*ns), clk.ctypes.data,
                                         (C.c_void_p * W)(*out_ptrs), (C.c_void_p * W)(*streams)), "gub_p2p_step_local_all")
+
+
+def _params_array(params):
+    params = np.ascontiguousarray(params)
+    assert params.dtype == PARAMS_DTYPE
+    return params
+
+
+def p2p_step_keys_local_all(p2ps, packed_ptrs, packed_bytes, ns, params, created_base, clk, out_ptrs, streams):
+    """p2p_step_local_all fed with key strings (gub_p2p_step_keys_local_all): packed_ptrs[r] = shard r's pack_keys() buffer on its device."""
+    W = len(p2ps)
+    params = _params_array(params)
+    _check(_entry("gub_p2p_step_keys_local_all")((C.c_void_p * W)(*[p._h for p in p2ps]), W, (C.c_void_p * W)(*packed_ptrs), (C.c_size_t * W)(*packed_bytes),
+                                             (C.c_size_t * W)(*ns), params.ctypes.data if len(params) else None, len(params), int(created_base),
+                                             clk.ctypes.data, (C.c_void_p * W)(*out_ptrs), (C.c_void_p * W)(*streams)), "gub_p2p_step_keys_local_all")
+
+
+def p2p_step_mixed_local_all(p2ps, req_ptrs, packed_ptrs, packed_bytes, ns, params, created_base, clk, out_ptrs, streams):
+    """Both kinds of ingest in one step (gub_p2p_step_mixed_local_all): shard r ingests key strings when packed_ptrs[r] is not None,
+    else the records at req_ptrs[r]."""
+    W = len(p2ps)
+    params = _params_array(params)
+    _check(_entry("gub_p2p_step_mixed_local_all")((C.c_void_p * W)(*[p._h for p in p2ps]), W, (C.c_void_p * W)(*req_ptrs), (C.c_void_p * W)(*packed_ptrs),
+                                              (C.c_size_t * W)(*packed_bytes), (C.c_size_t * W)(*ns), params.ctypes.data if len(params) else None,
+                                              len(params), int(created_base), clk.ctypes.data, (C.c_void_p * W)(*out_ptrs), (C.c_void_p * W)(*streams)),
+           "gub_p2p_step_mixed_local_all")
 
 
 def global_tick_local_all(p2ps, clk, now_ms, streams):

@@ -336,6 +336,30 @@ int gub_p2p_step_streams(gub_p2p* p, const gub_req* d_reqs, size_t n, const gub_
  * routings are enqueued, then all evaluations, then all collects.  streams[r] = the stream of shard r (on its device). */
 int gub_p2p_step_local_all(gub_p2p* const* ps, uint32_t world, const gub_req* const* d_reqs, const size_t* n, const gub_clock* clk,
                            gub_resp* const* d_out, void* const* streams);
+/* The ring fed with key strings: the step's ingest is a packed batch in the layout of gub_keys_layout ([gub_kreq x n][uint32 offsets
+ * x (n + 1)][key bytes]) in device memory on the shard's GPU, and `params` a host array as for gub_submit_keys_async.  One kernel,
+ * k_p2p_route_keys, hashes every key (XXH64 + FNV-1), expands its parameter set and created_at = created_base + created_delta
+ * (an unknown parameter index answers GUB_ERR_INVALID_ALGORITHM in-band) and routes the record exactly as gub_p2p_step would route
+ * the host-hashed one: same owner (by FNV-1, whatever the ring's hash_kind), same mailbox layout.  The rest of the step, GLOBAL
+ * handling and the tick are unchanged; stream semantics are those of gub_p2p_step_streams (pass the same stream twice for one stream).
+ * Offsets are not checked on the host (they live on the device); the kernel clamps them to the buffer: with key_bytes = packed_bytes -
+ * bytes_at, key i = bytes[lo .. hi) with hi = min(offsets[i + 1], key_bytes) and lo = min(offsets[i], hi), so a malformed entry is
+ * hashed as that (possibly empty) key and nothing outside the buffer is read.  packed_bytes must cover the records and offsets.
+ * More than 32 parameter sets are copied on the ingest stream into a device buffer of the gub_p2p (one per step parity); the buffer
+ * grows when a larger table arrives, which is the only allocation a step makes (and synchronises the device once).
+ * Mixing: the mailbox format is the same for both kinds of ingest, so in one step some shards may ingest key strings while others
+ * ingest records (gub_p2p_step_keys on some, gub_p2p_step on others; gub_p2p_step_mixed_local_all in one process).  The collective
+ * rule is unchanged: every shard steps once per step, whichever entry it uses. */
+int gub_p2p_step_keys(gub_p2p* p, const void* d_packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params,
+                      int64_t created_base, const gub_clock* clk, gub_resp* d_out, void* ingest_stream, void* stream);
+/* gub_p2p_step_local_all with key strings: shard r ingests d_packed[r] (packed_bytes[r], n[r] requests); one parameter table. */
+int gub_p2p_step_keys_local_all(gub_p2p* const* ps, uint32_t world, const void* const* d_packed, const size_t* packed_bytes, const size_t* n,
+                                const gub_params* params, size_t n_params, int64_t created_base, const gub_clock* clk,
+                                gub_resp* const* d_out, void* const* streams);
+/* Both in one step of the shards of this process: shard r ingests key strings when d_packed[r] != NULL, else the records d_reqs[r]. */
+int gub_p2p_step_mixed_local_all(gub_p2p* const* ps, uint32_t world, const gub_req* const* d_reqs, const void* const* d_packed,
+                                 const size_t* packed_bytes, const size_t* n, const gub_params* params, size_t n_params,
+                                 int64_t created_base, const gub_clock* clk, gub_resp* const* d_out, void* const* streams);
 /* Device-side waits are bounded (a dead peer must not hang the GPU); a wait that gave up marks the step: *error_out != 0 and the
  * call fails with text in gub_last_error().  Requests whose owner never answered carry GUB_ERR_PEER_TIMEOUT in-band.  Costs a
  * device synchronisation: poll at your own cadence. */
