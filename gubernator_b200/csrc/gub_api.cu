@@ -1225,10 +1225,19 @@ struct gub_p2p {
   } rt[2];
   // GLOBAL behaviour (gub_p2p_enable_global): device queues + tick buffers
   gub_gq *hits_q = nullptr, *updates_q = nullptr;
-  uint32_t gcap = 0;
+  uint32_t gq_recs = 0;            // next_pow2(capacity): the queues' size, and the most records / items one tick handles
+  uint32_t gcap = 0;               // min(gq_recs, cap): the items one NCCL all-gather slice carries per rank
+  // g_reqs: the hit records in round order, then the status queries; g_items: the drained hit records (before partitioning), then
+  // the UpdatePeerGlobal items
   gub_req *g_reqs = nullptr; gub_resp* g_resps = nullptr; gub_item *g_items = nullptr, *g_gather = nullptr;
   uint32_t* g_count = nullptr;     // [4] device counters (hits drained, queries drained, items made, spare)
   uint32_t* g_counts_all = nullptr;  // [MAX_SHARDS] device: items per rank
+  uint32_t* g_hist = nullptr;      // [GQ_BINS] device: this tick's hit records per bin, then the partition's cursors
+  uint32_t* g_hist_all = nullptr;  // [world x GQ_BINS] device: every rank's histogram (NCCL all-gather)
+  uint32_t* h_hist = nullptr;      // pinned [world x GQ_BINS]: row r = rank r's histogram (local group: only our own row is filled)
+  uint32_t* h_start = nullptr;     // pinned [GQ_BINS + 1]: exclusive prefix sum of our histogram
+  std::vector<gub::GqRound> rounds;  // the tick's rounds, identical on every shard
+  uint32_t round_n = 0;            // hit records this shard sends in the round in flight
   uint64_t seq = 0;
   // all shards in one process (gub_p2p_connect_local): peers by pointer + a host-side rendezvous for the GLOBAL tick
   struct LocalGroup { std::mutex mu; std::condition_variable cv; uint32_t arrived = 0, gen = 0; } own_group;
@@ -1265,9 +1274,12 @@ void gub_p2p_destroy(gub_p2p* p) {
   cudaSetDevice(p->t->device);
   cudaDeviceSynchronize();
   for (uint32_t r = 0; r < p->world; r++) if (p->opened[r]) cudaIpcCloseMemHandle(p->opened[r]);
-  void* ptrs[] = {p->block, p->error, p->ticket, p->seg_off, p->g_reqs, p->g_resps, p->g_items, p->g_gather, p->g_count, p->g_counts_all};
+  void* ptrs[] = {p->block, p->error, p->ticket, p->seg_off, p->g_reqs, p->g_resps, p->g_items, p->g_gather, p->g_count, p->g_counts_all,
+                  p->g_hist, p->g_hist_all};
   for (void* q : ptrs) if (q) cudaFree(q);
   if (p->h_counts) cudaFreeHost(p->h_counts);
+  if (p->h_hist) cudaFreeHost(p->h_hist);
+  if (p->h_start) cudaFreeHost(p->h_start);
   if (p->phase_ev) cudaEventDestroy(p->phase_ev);
   if (p->ev_fork) cudaEventDestroy(p->ev_fork);
   if (p->s_eval) cudaStreamDestroy(p->s_eval);
@@ -1854,7 +1866,10 @@ int gub_p2p_nccl_init_local(gub_p2p* const* ps, uint32_t world) {
 
 /* Turns GLOBAL handling on for this shard's steps: GLOBAL requests it does not own are answered from the local replica
  * (gubernator.go:257-269,408-411) and their hits queued (global.go:74-111); GLOBAL requests it evaluates as owner are queued for
- * the broadcast (global.go:80-84,201).  capacity = most distinct GLOBAL keys per sync window (drops are counted in gq_dropped). */
+ * the broadcast (global.go:80-84,201).  capacity = most distinct GLOBAL keys per sync window, rounded up to a power of two Q; a tick
+ * carries all of them (in rounds when they exceed the mailbox capacity), and only requests that find the queue full are counted in
+ * gq_dropped.  Device memory per shard: the two queues, (64 + 32 + 88) B x Q of tick staging, a 256 KiB histogram, world x 256 KiB
+ * for the histogram exchange and 88 B x min(Q, cap) x world for the item all-gather; (world + 1) x 256 KiB of pinned host memory. */
 int gub_p2p_enable_global(gub_p2p* p, uint32_t capacity) {
   if (!p || capacity < 64) return fail("gub_p2p_enable_global: bad argument");
   if (p->hits_q) return 0;
@@ -1863,17 +1878,25 @@ int gub_p2p_enable_global(gub_p2p* p, uint32_t capacity) {
   if (gub_gq_create(p->t->device, capacity, 1, &p->updates_q)) return -1;
   p->hits_q->q.dropped = p->t->counters + gub::C_GQ_DROPPED;
   p->updates_q->q.dropped = p->t->counters + gub::C_GQ_DROPPED;
-  p->gcap = std::min<uint32_t>(next_pow2(capacity), p->cap);
-  CK(cudaMalloc(&p->g_reqs, (size_t)p->gcap * sizeof(gub_req)));
-  CK(cudaMalloc(&p->g_resps, (size_t)p->gcap * sizeof(gub_resp)));
-  CK(cudaMalloc(&p->g_items, (size_t)p->gcap * sizeof(gub_item)));
+  p->gq_recs = next_pow2(capacity);
+  p->gcap = std::min<uint32_t>(p->gq_recs, p->cap);
+  static_assert(sizeof(gub_item) >= sizeof(gub_req), "g_items also holds the drained hit records");
+  CK(cudaMalloc(&p->g_reqs, (size_t)p->gq_recs * sizeof(gub_req)));
+  CK(cudaMalloc(&p->g_resps, (size_t)p->gq_recs * sizeof(gub_resp)));
+  CK(cudaMalloc(&p->g_items, (size_t)p->gq_recs * sizeof(gub_item)));
   CK(cudaMalloc(&p->g_gather, (size_t)p->gcap * p->world * sizeof(gub_item)));
   CK(cudaMalloc(&p->g_count, 16));
   CK(cudaMemset(p->g_count, 0, 16));
   CK(cudaMalloc(&p->g_counts_all, gub::MAX_SHARDS * 4));
+  CK(cudaMalloc(&p->g_hist, (size_t)gub::GQ_BINS * 4));
+  CK(cudaMalloc(&p->g_hist_all, (size_t)gub::GQ_BINS * 4 * p->world));
   for (auto& r : p->rt) CK(cudaMalloc(&r.expanded, (size_t)p->cap * sizeof(gub_req)));
   CK(cudaHostAlloc(&p->h_counts, 16, cudaHostAllocDefault));
   std::memset(p->h_counts, 0, 16);
+  CK(cudaHostAlloc(&p->h_hist, (size_t)gub::GQ_BINS * 4 * p->world, cudaHostAllocDefault));
+  std::memset(p->h_hist, 0, (size_t)gub::GQ_BINS * 4 * p->world);
+  CK(cudaHostAlloc(&p->h_start, ((size_t)gub::GQ_BINS + 1) * 4, cudaHostAllocDefault));
+  std::memset(p->h_start, 0, ((size_t)gub::GQ_BINS + 1) * 4);
   if (gq_reserve(p->updates_q, (size_t)p->world * p->cap, 0)) return -1;
   if (gq_reserve(p->hits_q, p->cap, 0)) return -1;
   return 0;
@@ -1884,17 +1907,24 @@ int gub_p2p_enable_global(gub_p2p* p, uint32_t capacity) {
  * all-gather when the shard has a communicator (one process per GPU); direct peer reads when all shards live in this process
  * (gub_p2p_connect_local), where the calling threads — one per shard — rendezvous on the host.  Collective: every shard of the
  * ring calls it the same number of times, interleaved the same way with its steps.  now_ms = MillisecondNow() of the receivers
- * (CreatedAt / UpdatedAt of the installed items).  The one host round trip is the per-shard item counts (a tick runs every
- * GlobalSyncWait = 500 ms, not per batch).
+ * (CreatedAt / UpdatedAt of the installed items).
+ * The window's hit records travel in key-consistent rounds of at most `cap` records per source, one mailbox epoch each (see
+ * gub_global.cuh): every shard's histogram of its records over the hash space reaches every shard (read in place inside one
+ * process, all-gathered by NCCL across processes), and every shard derives the same rounds from them.  Two host round trips: the
+ * histograms, then the per-shard item counts (a tick runs every GlobalSyncWait = 500 ms, not per batch).
  * stats (optional, 4 x uint64): hit records sent to owners, update items broadcast by this shard, items installed here, bytes moved. */
 }  // extern "C"
 
 namespace {
 
-// A tick in three enqueue-only phases (no host synchronisation inside), so that one host thread can drive all the shards of a
-// process phase by phase (see gub_p2p_step_local_all).
-// A: the window's aggregated hits -> their owners' mailboxes (plain routing: these records go to the owner).
-int tick_phase_a(gub_p2p* p, cudaStream_t st) {
+// A tick in enqueue-only pieces (the drivers synchronise between them), so that one host thread can drive all the shards of a
+// process piece by piece (see gub_p2p_step_local_all).
+// The drained hit records wait in g_items until k_gq_partition has put them in round order; the items come later.
+gub_req* hit_stage(gub_p2p* p) { return reinterpret_cast<gub_req*>(p->g_items); }
+
+// The window's aggregated hits, drained and counted per bin.  Our histogram lands in our row of h_hist; with `gather` (NCCL) every
+// rank's histogram lands in h_hist.
+int tick_drain_hits(gub_p2p* p, bool gather, cudaStream_t st) {
   gub_table* t = p->t;
   std::lock_guard<std::mutex> lk(t->mu);
   CK(cudaSetDevice(t->device));
@@ -1906,16 +1936,50 @@ int tick_phase_a(gub_p2p* p, cudaStream_t st) {
       CK(cudaStreamWaitEvent(st, p->ev_fork, 0));
     }
   }
+  const size_t row = (size_t)gub::GQ_BINS * 4;
   CK(cudaMemsetAsync(p->g_count, 0, 16, st));
-  gub::k_gq_drain<<<p->t->num_sms, 256, 0, st>>>(p->hits_q->q, p->g_reqs, p->gcap, p->g_count + 0, 0u);
+  CK(cudaMemsetAsync(p->g_hist, 0, row, st));
+  gub::k_gq_drain<<<t->num_sms, 256, 0, st>>>(p->hits_q->q, hit_stage(p), p->gq_recs, p->g_count + 0, 0u);
+  gub::k_gq_hist<<<t->num_sms, 256, 0, st>>>(hit_stage(p), p->gq_recs, p->g_count + 0, p->g_hist);
+  CK(cudaGetLastError());
+  if (gather) {
+    NCK(g_nccl.AllGather(p->g_hist, p->g_hist_all, gub::GQ_BINS, /* ncclUint32 */ 3, p->nccl, st));
+    CK(cudaMemcpyAsync(p->h_hist, p->g_hist_all, row * p->world, cudaMemcpyDeviceToHost, st));
+  } else {
+    CK(cudaMemcpyAsync(p->h_hist + (size_t)p->rank * gub::GQ_BINS, p->g_hist, row, cudaMemcpyDeviceToHost, st));
+  }
+  return 0;
+}
+
+// Our drained records in round order (g_reqs), by a counting sort over the bins; `own` = our histogram (host).
+int tick_partition(gub_p2p* p, const uint32_t* own, cudaStream_t st) {
+  gub_table* t = p->t;
+  std::lock_guard<std::mutex> lk(t->mu);
+  CK(cudaSetDevice(t->device));
+  p->h_start[0] = 0;
+  for (uint32_t b = 0; b < gub::GQ_BINS; b++) p->h_start[b + 1] = p->h_start[b] + own[b];
+  // the histogram has reached the host (and the NCCL all-gather): its device buffer becomes the partition's cursors
+  CK(cudaMemcpyAsync(p->g_hist, p->h_start, (size_t)gub::GQ_BINS * 4, cudaMemcpyHostToDevice, st));
+  gub::k_gq_partition<<<t->num_sms, 256, 0, st>>>(hit_stage(p), p->gq_recs, p->g_count + 0, p->g_hist, p->g_reqs);
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// Round i, routed: our records of that round -> their owners' mailboxes (plain routing: these records go to the owner).
+int tick_round_route(gub_p2p* p, size_t i, cudaStream_t st) {
+  gub_table* t = p->t;
+  std::lock_guard<std::mutex> lk(t->mu);
+  CK(cudaSetDevice(t->device));
+  uint32_t off = 0;
+  gub::gq_round_span(p->rounds[i], p->h_start, p->cap, &off, &p->round_n);
   p->epoch++;
   gub_p2p::Route* rt = &p->rt[p->epoch & 1u];
   if (rt->step_done_valid) CK(cudaStreamWaitEvent(st, rt->step_done, 0));
   gub::P2PArgs A;
   p2p_args(p, A);
-  return p2p_route(p, rt, A, p->g_reqs, p->gcap, p->g_count + 0, -1, st);
+  return p2p_route(p, rt, A, p->g_reqs + off, p->round_n, nullptr, -1, st);
 }
-// B: owners apply the hits with DRAIN_OVER_LIMIT as owner (gubernator.go:510-512).
+// Owners apply the round's hits with DRAIN_OVER_LIMIT as owner (gubernator.go:510-512).
 int tick_phase_b(gub_p2p* p, const gub_clock* clk, cudaStream_t st) {
   gub_table* t = p->t;
   std::lock_guard<std::mutex> lk(t->mu);
@@ -1929,32 +1993,34 @@ int tick_phase_b(gub_p2p* p, const gub_clock* clk, cudaStream_t st) {
   CK(cudaGetLastError());
   return 0;
 }
-// C: owners re-read every key touched by GLOBAL traffic with Hits = 0 (global.go:243-245) and build the UpdatePeerGlobal items.
-int tick_phase_c(gub_p2p* p, const gub_clock* clk, cudaStream_t st) {
+// The owners' answers to our hit records are dropped (sendHits ignores them), but the flags are consumed: epochs stay aligned.
+// (Enqueued after EVERY shard's evaluation of the round: on a device shared by several shards a collect spinning ahead of another
+// shard's batch kernel would keep that cooperative kernel from ever becoming resident.)
+int tick_round_collect(gub_p2p* p, cudaStream_t st) {
   gub_table* t = p->t;
   std::lock_guard<std::mutex> lk(t->mu);
   CK(cudaSetDevice(t->device));
-  {  // the owners' answers to our hit records are dropped (sendHits ignores them), but the flags are consumed: epochs stay aligned.
-     // (Enqueued here, after EVERY shard's evaluation: on a device shared by several shards a collect spinning ahead of another
-     // shard's batch kernel would keep that cooperative kernel from ever becoming resident.)
-    gub_p2p::Route* rt = &p->rt[p->epoch & 1u];
-    gub::P2PArgs A;
-    p2p_args(p, A);
-    gub::k_p2p_collect<<<64, 256, 0, st>>>(A, rt->perm, p->gcap, p->g_count + 0, p->g_resps);
-    CK(cudaEventRecord(rt->step_done, st)); rt->step_done_valid = true;
-    p->seq += (uint64_t)1 << 32;
-  }
-  gub::k_gq_drain<<<p->t->num_sms, 256, 0, st>>>(p->updates_q->q, p->g_reqs, p->gcap, p->g_count + 1, 1u);
-  if (launch_batch(t, p->g_reqs, p->gcap, clk, p->g_resps, st, p->g_count + 1)) return -1;  // (either kernel path; the count lives on the device)
-  gub::k_make_updates<<<(p->gcap + 255) / 256, 256, 0, st>>>(p->g_reqs, p->g_resps, p->gcap, p->g_count + 1, p->g_items, p->g_count + 2);
+  gub_p2p::Route* rt = &p->rt[p->epoch & 1u];
+  gub::P2PArgs A;
+  p2p_args(p, A);
+  gub::k_p2p_collect<<<64, 256, 0, st>>>(A, rt->perm, p->round_n, nullptr, p->g_resps);
+  CK(cudaEventRecord(rt->step_done, st)); rt->step_done_valid = true;
+  CK(cudaGetLastError());
+  p->seq += (uint64_t)1 << 32;
+  return 0;
+}
+// Owners re-read every key touched by GLOBAL traffic with Hits = 0 (global.go:243-245) and build the UpdatePeerGlobal items.
+int tick_updates(gub_p2p* p, const gub_clock* clk, cudaStream_t st) {
+  gub_table* t = p->t;
+  std::lock_guard<std::mutex> lk(t->mu);
+  CK(cudaSetDevice(t->device));
+  const uint32_t Q = p->gq_recs;
+  gub::k_gq_drain<<<t->num_sms, 256, 0, st>>>(p->updates_q->q, p->g_reqs, Q, p->g_count + 1, 1u);
+  if (launch_batch(t, p->g_reqs, Q, clk, p->g_resps, st, p->g_count + 1)) return -1;  // (either kernel path; chunked; the count lives on the device)
+  gub::k_make_updates<<<(Q + 255) / 256, 256, 0, st>>>(p->g_reqs, p->g_resps, Q, p->g_count + 1, p->g_items, p->g_count + 2);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(p->h_counts, p->g_count, 16, cudaMemcpyDeviceToHost, st));
   return 0;
-}
-int tick_enqueue(gub_p2p* p, const gub_clock* clk, cudaStream_t st) {
-  if (tick_phase_a(p, st)) return -1;
-  if (tick_phase_b(p, clk, st)) return -1;
-  return tick_phase_c(p, clk, st);
 }
 
 void group_barrier(gub_p2p::LocalGroup* g, uint32_t world) {
@@ -1962,6 +2028,33 @@ void group_barrier(gub_p2p::LocalGroup* g, uint32_t world) {
   const uint32_t my = g->gen;
   if (++g->arrived == world) { g->arrived = 0; g->gen++; g->cv.notify_all(); }
   else g->cv.wait(lk, [&] { return g->gen != my; });
+}
+
+// local_phase_sync for one thread per shard: our stream waits for the piece every other shard has just enqueued.  Reaches both
+// barriers whatever happens, so that a failing shard does not leave its peers waiting.
+int group_phase_sync(gub_p2p* p, cudaStream_t st) {
+  bool ok = cudaSetDevice(p->t->device) == cudaSuccess;
+  if (ok && !p->phase_ev) ok = cudaEventCreateWithFlags(&p->phase_ev, cudaEventDisableTiming) == cudaSuccess;
+  if (ok) ok = cudaEventRecord(p->phase_ev, st) == cudaSuccess;
+  group_barrier(p->group, p->world);
+  for (uint32_t q = 0; q < p->world; q++) {
+    if (ok && q != p->rank) ok = p->local_peers[q]->phase_ev && cudaStreamWaitEvent(st, p->local_peers[q]->phase_ev, 0) == cudaSuccess;
+  }
+  group_barrier(p->group, p->world);  // nobody records its event again before every peer has waited on it
+  return ok ? 0 : fail("gub_global_tick: ordering the shards' streams failed");
+}
+
+// The rounds of one shard, driven by its own thread (with `group`: the shards of this process rendezvous between the pieces).
+// rc != 0: an earlier piece failed; nothing more is enqueued, but the rendezvous still happen.
+int tick_rounds(gub_p2p* p, const gub_clock* clk, cudaStream_t st, bool group, int rc) {
+  for (size_t i = 0; i < p->rounds.size(); i++) {
+    if (!rc) rc = tick_round_route(p, i, st);
+    if (group && group_phase_sync(p, st)) rc = -1;
+    if (!rc) rc = tick_phase_b(p, clk, st);
+    if (group && group_phase_sync(p, st)) rc = -1;
+    if (!rc) rc = tick_round_collect(p, st);
+  }
+  return rc;
 }
 
 // Installs the items every other shard of this process has made (their g_items, read in place: same device or peer memory).
@@ -1973,7 +2066,7 @@ int tick_install_local(gub_p2p* p, int64_t now_ms, cudaStream_t st, uint64_t* in
   for (uint32_t r = 0; r < p->world; r++) {
     if (r == p->rank) continue;  // "Exclude ourselves from the update" (global.go:263-265)
     const gub_p2p* q = p->local_peers[r];
-    const uint32_t k = std::min(q->h_counts[2], q->gcap);
+    const uint32_t k = std::min(q->h_counts[2], q->gq_recs);
     if (!k) continue;
     gub::k_add_items_pub<<<(k + 255) / 256, 256, 0, st>>>(t->table, t->capacity, q->g_items, k, now_ms, t->counters, t->inv);
     *installed += k;
@@ -1988,19 +2081,22 @@ int tick_install_nccl(gub_p2p* p, int64_t now_ms, cudaStream_t st, uint64_t* ins
   gub_table* t = p->t;
   std::lock_guard<std::mutex> lk(t->mu);
   CK(cudaSetDevice(t->device));
-  // all-gather: counts first (the host needs them to size the item gather), then the items, padded to the largest count
+  // all-gather: counts first (the host needs them to size the item gathers), then the items in slices of gcap per rank, each padded
+  // to the largest count of its slice (g_gather stays gcap x world items)
   std::vector<uint32_t> all(p->world, 0);
   NCK(g_nccl.AllGather(p->g_count + 2, p->g_counts_all, 1, /* ncclUint32 */ 3, p->nccl, st));
   CK(cudaMemcpyAsync(all.data(), p->g_counts_all, p->world * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  uint32_t pad = 0;
-  for (uint32_t r = 0; r < p->world; r++) pad = std::max(pad, std::min(all[r], p->gcap));
+  auto slice = [&](uint32_t r, uint32_t base) { const uint32_t k = std::min(all[r], p->gq_recs); return k > base ? std::min(k - base, p->gcap) : 0u; };
   p->tick_bytes = 0;
-  if (pad) {
-    NCK(g_nccl.AllGather(p->g_items, p->g_gather, (size_t)pad * sizeof(gub_item), /* ncclUint8 */ 1, p->nccl, st));
-    p->tick_bytes = (uint64_t)pad * sizeof(gub_item) * p->world;
+  for (uint32_t base = 0;; base += p->gcap) {
+    uint32_t pad = 0;
+    for (uint32_t r = 0; r < p->world; r++) pad = std::max(pad, slice(r, base));
+    if (!pad) break;
+    NCK(g_nccl.AllGather(p->g_items + base, p->g_gather, (size_t)pad * sizeof(gub_item), /* ncclUint8 */ 1, p->nccl, st));
+    p->tick_bytes += (uint64_t)pad * sizeof(gub_item) * p->world;
     for (uint32_t r = 0; r < p->world; r++) {
-      const uint32_t k = std::min(all[r], p->gcap);
+      const uint32_t k = slice(r, base);
       if (r == p->rank || !k) continue;  // "Exclude ourselves from the update" (global.go:263-265)
       gub::k_add_items_pub<<<(k + 255) / 256, 256, 0, st>>>(t->table, t->capacity, p->g_gather + (size_t)r * pad, k, now_ms, t->counters, t->inv);
       *installed += k;
@@ -2012,7 +2108,7 @@ int tick_install_nccl(gub_p2p* p, int64_t now_ms, cudaStream_t st, uint64_t* ins
 
 void tick_stats(gub_p2p* p, uint64_t installed, uint64_t* stats) {
   if (!stats) return;
-  stats[0] = std::min(p->h_counts[0], p->gcap); stats[1] = std::min(p->h_counts[2], p->gcap); stats[2] = installed; stats[3] = p->tick_bytes;
+  stats[0] = std::min(p->h_counts[0], p->gq_recs); stats[1] = std::min(p->h_counts[2], p->gq_recs); stats[2] = installed; stats[3] = p->tick_bytes;
 }
 
 }  // namespace
@@ -2024,36 +2120,57 @@ int gub_global_tick(gub_p2p* p, const gub_clock* clk, int64_t now_ms, void* stre
   if (!p->hits_q) return fail("gub_global_tick: gub_p2p_enable_global has not been called");
   if (p->world > 1 && !p->nccl && !p->group) return fail("gub_global_tick: no NCCL communicator (gub_p2p_nccl_init) and the shards are not local to this process");
   cudaStream_t st = (cudaStream_t)stream;
-  if (tick_enqueue(p, clk, st)) return -1;
+  const bool nccl = p->world > 1 && p->nccl, group = p->world > 1 && !nccl;
+  // From here on a shard of a local group reaches every rendezvous even when a piece fails, so that its peers do not wait forever.
+  int rc = tick_drain_hits(p, nccl, st);
+  if (!rc && (cudaSetDevice(p->t->device) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)) rc = fail("gub_global_tick: the hit histogram did not arrive");
+  if (group) group_barrier(p->group, p->world);  // every shard's histogram is on the host
+  std::vector<const uint32_t*> rows(p->world);
+  for (uint32_t q = 0; q < p->world; q++) rows[q] = (group ? p->local_peers[q]->h_hist : p->h_hist) + (size_t)q * gub::GQ_BINS;
+  gub::gq_plan_rounds(rows.data(), p->world, p->cap, p->rounds);
+  if (!rc) rc = tick_partition(p, rows[p->rank], st);
+  rc = tick_rounds(p, clk, st, group, rc);
+  if (!rc) rc = tick_updates(p, clk, st);
   uint64_t installed = 0;
-  if (p->world > 1 && p->nccl) {
-    if (tick_install_nccl(p, now_ms, st, &installed)) return -1;
-    CK(cudaStreamSynchronize(st));
+  if (nccl) {
+    if (!rc) rc = tick_install_nccl(p, now_ms, st, &installed);
+    if (!rc) CK(cudaStreamSynchronize(st));
   } else {
-    CK(cudaSetDevice(p->t->device));
-    CK(cudaStreamSynchronize(st));  // my items and their count are final
-    if (p->world > 1) {
+    if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = fail("gub_global_tick: the tick failed on the device");  // my items and their count are final
+    if (group) {
       group_barrier(p->group, p->world);  // ... and so are everybody else's
-      const int rc = tick_install_local(p, now_ms, st, &installed);
+      if (!rc) rc = tick_install_local(p, now_ms, st, &installed);
       group_barrier(p->group, p->world);  // nobody still reads my items
-      if (rc) return -1;
     }
   }
+  if (rc) return -1;
   tick_stats(p, installed, stats);
   return 0;
 }
 
-/* The same for a single host thread driving all the shards of this process (gub_p2p_connect_local): phases run shard by shard. */
+/* The same for a single host thread driving all the shards of this process (gub_p2p_connect_local): pieces run shard by shard. */
 int gub_global_tick_local_all(gub_p2p* const* ps, uint32_t world, const gub_clock* clk, int64_t now_ms, void* const* streams, uint64_t* stats /* world x 4, optional */) {
   if (!ps || !clk || !streams || world == 0) return fail("gub_global_tick_local_all: bad argument");
   for (uint32_t r = 0; r < world; r++) {
     if (!ps[r] || !ps[r]->hits_q || ps[r]->world != world || (world > 1 && !ps[r]->group)) return fail("gub_global_tick_local_all: shards must be local, connected and GLOBAL-enabled");
   }
-  for (uint32_t r = 0; r < world; r++) if (tick_phase_a(ps[r], (cudaStream_t)streams[r])) return -1;
-  if (local_phase_sync(ps, world, streams)) return -1;
-  for (uint32_t r = 0; r < world; r++) if (tick_phase_b(ps[r], clk, (cudaStream_t)streams[r])) return -1;
-  if (local_phase_sync(ps, world, streams)) return -1;
-  for (uint32_t r = 0; r < world; r++) if (tick_phase_c(ps[r], clk, (cudaStream_t)streams[r])) return -1;
+  for (uint32_t r = 0; r < world; r++) if (tick_drain_hits(ps[r], false, (cudaStream_t)streams[r])) return -1;
+  for (uint32_t r = 0; r < world; r++) { CK(cudaSetDevice(ps[r]->t->device)); CK(cudaStreamSynchronize((cudaStream_t)streams[r])); }
+  std::vector<const uint32_t*> rows(world);
+  for (uint32_t q = 0; q < world; q++) rows[q] = ps[q]->h_hist + (size_t)q * gub::GQ_BINS;
+  gub::gq_plan_rounds(rows.data(), world, ps[0]->cap, ps[0]->rounds);
+  for (uint32_t r = 0; r < world; r++) {
+    ps[r]->rounds = ps[0]->rounds;
+    if (tick_partition(ps[r], rows[r], (cudaStream_t)streams[r])) return -1;
+  }
+  for (size_t i = 0; i < ps[0]->rounds.size(); i++) {
+    for (uint32_t r = 0; r < world; r++) if (tick_round_route(ps[r], i, (cudaStream_t)streams[r])) return -1;
+    if (local_phase_sync(ps, world, streams)) return -1;
+    for (uint32_t r = 0; r < world; r++) if (tick_phase_b(ps[r], clk, (cudaStream_t)streams[r])) return -1;
+    if (local_phase_sync(ps, world, streams)) return -1;
+    for (uint32_t r = 0; r < world; r++) if (tick_round_collect(ps[r], (cudaStream_t)streams[r])) return -1;
+  }
+  for (uint32_t r = 0; r < world; r++) if (tick_updates(ps[r], clk, (cudaStream_t)streams[r])) return -1;
   for (uint32_t r = 0; r < world; r++) { CK(cudaSetDevice(ps[r]->t->device)); CK(cudaStreamSynchronize((cudaStream_t)streams[r])); }
   for (uint32_t r = 0; r < world; r++) {
     uint64_t installed = 0;

@@ -7,12 +7,16 @@
 //           state with Hits = 0 (global.go:243-245) and broadcasts it; peers overwrite their replica (UpdatePeerGlobals).
 // Here both maps are one device structure, a `gq`: an open-addressed table of 64-byte gub_req records keyed by the
 // request's XXH64, filled by two small kernels per batch (claim: insert / sum hits / order by sequence; fill: the winning
-// request writes its parameters) and drained into a dense array of request records at each sync tick.
+// request writes its parameters) and drained into a dense array of request records at each sync tick, which sends the hit
+// records to their owners in key-consistent rounds (k_gq_hist, gq_plan_rounds, k_gq_partition below).
 #pragma once
 #if !defined(GUB_EMULATE)  // tests/kernel_emu_harness.cpp compiles this header for the CPU (see gub_kernels.cuh)
 #include <cuda_runtime.h>
 #endif
 #include <stdint.h>
+
+#include <algorithm>
+#include <vector>
 
 #include "../../include/gubernator_b200.h"
 
@@ -140,13 +144,90 @@ __global__ void k_gq_drain(Gq q, gub_req* out, uint32_t out_cap, uint32_t* out_c
       else e.behavior |= (uint32_t)(GUB_BEHAVIOR_DRAIN_OVER_LIMIT | GUB_REQ_IS_OWNER);
       out[k] = e;
     } else if (q.dropped) {
-      atomicAdd(q.dropped, 1ull);  // more keys in one sync window than a tick carries (the mailbox capacity): counted, not silent
+      atomicAdd(q.dropped, 1ull);  // an output smaller than the queue (gub_gq_drain_device); the sync tick drains into the queue's capacity
     }
     gub_req z = {};
     q.slots[pos] = z;
     q.seq[pos] = 0ull;
   }
   if (blockIdx.x == 0 && threadIdx.x == 0) *q.count = 0ull;
+}
+
+// ---- A sync tick's hit records in rounds ----------------------------------------------------------------------------------------
+// A tick sends every drained hit record to its owner through the ring's mailboxes, which take at most `cap` records per source and
+// step.  A window of more keys travels in rounds, one mailbox epoch each.  The rounds are key-consistent: the hash space is cut
+// into GQ_BINS bins by the top 16 bits of key_xxh64, and consecutive bins are packed into rounds such that no source has more than
+// `cap` records in one round.  Every source's record of a key therefore travels in the same round, and the owner applies them in
+// source-rank order, exactly as a single-round tick (and OracleCluster.tick of tests/global_model.py) does.  The packing is a
+// function of every shard's histogram alone, so every shard computes the same rounds.
+// A bin that holds more than `cap` records of one source (only crafted keys sharing their top 16 bits of XXH64 do that) is split by
+// position over consecutive rounds: nothing is dropped, but for those keys the order between sources is the round order.  The
+// reference defines no order between its peers' sendHits either.
+enum : uint32_t { GQ_BIN_BITS = 16, GQ_BINS = 1u << GQ_BIN_BITS };
+
+__device__ __forceinline__ uint32_t gq_bin(unsigned long long key) { return (uint32_t)(key >> (64 - GQ_BIN_BITS)); }
+
+// hist[bin] += records of that bin (hist zeroed by the caller).
+__global__ void k_gq_hist(const gub_req* recs, uint32_t n, const uint32_t* n_dev, uint32_t* hist) {
+  if (n_dev) n = min(n, *n_dev);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    atomicAdd(&hist[gq_bin(__ldg(reinterpret_cast<const unsigned long long*>(&recs[i].key_xxh64)))], 1u);
+}
+
+// Counting sort by bin: cursor[bin] = the first output index of that bin (the exclusive prefix sum of k_gq_hist), advanced here.
+// The order inside a bin is arbitrary; one source's records of one round are distinct keys, so it does not matter.
+__global__ void k_gq_partition(const gub_req* recs, uint32_t n, const uint32_t* n_dev, uint32_t* cursor, gub_req* out) {
+  if (n_dev) n = min(n, *n_dev);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const ulonglong2* p = reinterpret_cast<const ulonglong2*>(recs + i);
+    const ulonglong2 a = __ldg(p), b = __ldg(p + 1), c = __ldg(p + 2), d = __ldg(p + 3);
+    ulonglong2* o = reinterpret_cast<ulonglong2*>(out + atomicAdd(&cursor[gq_bin(a.x)], 1u));
+    o[0] = a; o[1] = b; o[2] = c; o[3] = d;
+  }
+}
+
+// One round: the bins [lo, hi); for a split bin (hi = lo + 1) slice k carries records k*cap ... k*cap + cap - 1 of every source.
+struct GqRound { uint32_t lo, hi, slice; };
+
+// Host side, identical on every shard.  hist[s] = source s's GQ_BINS counts.  Empty bins join a neighbouring round; an empty window
+// is one (empty) round, like the single-round tick.
+inline void gq_plan_rounds(const uint32_t* const* hist, uint32_t nsrc, uint32_t cap, std::vector<GqRound>& out) {
+  out.clear();
+  std::vector<uint64_t> sum(nsrc, 0);
+  uint32_t lo = 0;
+  bool open = false;
+  auto close = [&](uint32_t hi) {
+    if (open) out.push_back(GqRound{lo, hi, 0});
+    std::fill(sum.begin(), sum.end(), 0);
+    open = false;
+    lo = hi;
+  };
+  for (uint32_t b = 0; b < GQ_BINS; b++) {
+    uint32_t most = 0;
+    for (uint32_t s = 0; s < nsrc; s++) most = std::max(most, hist[s][b]);
+    if (most == 0) continue;
+    if (most > cap) {  // over-full bin: split by position
+      close(b);
+      for (uint32_t k = 0; k < (most + cap - 1) / cap; k++) out.push_back(GqRound{b, b + 1, k});
+      lo = b + 1;
+      continue;
+    }
+    bool fits = true;
+    for (uint32_t s = 0; s < nsrc; s++) fits = fits && sum[s] + hist[s][b] <= cap;
+    if (!fits) close(b);
+    for (uint32_t s = 0; s < nsrc; s++) sum[s] += hist[s][b];
+    open = true;
+  }
+  close(GQ_BINS);
+  if (out.empty()) out.push_back(GqRound{0, GQ_BINS, 0});
+}
+
+// This source's records of round R in the partitioned array: start = the exclusive prefix sum of its histogram (GQ_BINS + 1).
+inline void gq_round_span(const GqRound& R, const uint32_t* start, uint32_t cap, uint32_t* off, uint32_t* n) {
+  const uint32_t total = start[R.hi] - start[R.lo];
+  const uint64_t skip = std::min<uint64_t>((uint64_t)R.slice * cap, total);
+  *off = start[R.lo] + (uint32_t)skip;
+  *n = (uint32_t)std::min<uint64_t>(cap, total - skip);
 }
 
 // UpdatePeerGlobal records (peers.proto:52-72) from the owner's status queries: the CacheItem a peer will install

@@ -54,7 +54,8 @@ class ShardedStep:
 
     def tick(self, clk, now_ms):
         """One GLOBAL sync: sendHits (global.go:144-190) then broadcastPeers (global.go:234-283).  Collective: every rank
-        must call it.  Returns (hit records sent, update items received)."""
+        must call it.  Returns (hit records sent, update items received).  The window's hits travel in one all-to-all (a
+        single round); the ring's gub_global_tick is the one that splits a window larger than its mailboxes into rounds."""
         be, dist, W = self.be, self.dist, self.world
         self.steps += 1
         # 1. aggregated hits -> owners (GetPeerRateLimits on the owner: DRAIN_OVER_LIMIT, IsOwner = true)

@@ -122,7 +122,8 @@ typedef struct {
   uint64_t serial_fallbacks; /* chunks (<= 512 requests) of such groups that were mostly one-request runs: applied one by one */
   uint64_t unexpired_evictions; /* live entries displaced because a probe window was full: metricCacheUnexpiredEvictions (lrucache.go:138-149) */
   uint64_t swept;          /* removed / expired entries freed by the incremental sweep inside the batch kernel */
-  uint64_t gq_dropped;     /* GLOBAL requests not queued because a gub_gq was full within one sync window */
+  uint64_t gq_dropped;     /* GLOBAL requests not queued because a gub_gq was full within one sync window (queue overflow only:
+                              a sync tick carries every queued key) */
 } gub_counters;
 
 typedef struct {
@@ -369,11 +370,20 @@ int gub_p2p_status(gub_p2p* p, int* error_out);
  * requests this shard does not own from the local replica (GLOBAL cleared, NO_BATCHING set, IsOwner = false) and queues their
  * hits; GLOBAL requests evaluated as owner are queued for the broadcast.  gub_global_tick is the reference's GlobalSyncWait
  * timer made explicit: hits go to their owners (applied with DRAIN_OVER_LIMIT), owners re-read the touched keys with Hits = 0,
- * and an NCCL all-gather delivers the UpdatePeerGlobal items to every other shard, which overwrites its replica. */
+ * and an NCCL all-gather delivers the UpdatePeerGlobal items to every other shard, which overwrites its replica.
+ * capacity = most distinct GLOBAL keys per sync window, rounded up to a power of two Q; every tick carries all the keys the queues
+ * accepted.  Device memory per shard: the two queues, (64 + 32 + 88) B x Q of tick staging, a 256 KiB histogram, world x 256 KiB
+ * for the histogram exchange and 88 B x min(Q, mailbox capacity) x world for the item all-gather. */
 int gub_p2p_enable_global(gub_p2p* p, uint32_t capacity /* most distinct GLOBAL keys per sync window */);
 int gub_nccl_unique_id(void* out128 /* 128 bytes: ncclUniqueId, to be handed to every shard by the host application */);
 int gub_p2p_nccl_init(gub_p2p* p, const void* id128);                     /* one process per GPU; collective */
 int gub_p2p_nccl_init_local(gub_p2p* const* ps, uint32_t world);           /* all shards in this process */
+/* A window of more hit records than the mailboxes take (the capacity given to gub_p2p_create, per source) travels in rounds, one
+ * mailbox epoch each.  The rounds are key-consistent: every source's record of a key travels in the same round, so an owner applies
+ * them in source-rank order, as a single-round tick does.  Every shard's histogram of its records over the top 16 bits of XXH64
+ * reaches every shard (one added host synchronisation per tick), and all shards derive the same rounds from it.  Keys crafted to
+ * share their top 16 bits beyond that capacity are split over consecutive rounds: none is dropped, but for those keys the order
+ * between sources is the round order. */
 int gub_global_tick(gub_p2p* p, const gub_clock* clk, int64_t now_ms, void* stream, uint64_t* stats /* optional, 4 values */);
 /* All shards in this process, driven by ONE host thread (gub_global_tick itself expects one calling thread per local shard). */
 int gub_global_tick_local_all(gub_p2p* const* ps, uint32_t world, const gub_clock* clk, int64_t now_ms, void* const* streams,
