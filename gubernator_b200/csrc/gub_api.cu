@@ -38,6 +38,7 @@ int fail(const std::string& msg) { g_err = msg; return -1; }
   } while (0)
 
 constexpr int PIPE_DEPTH = 4;
+constexpr uint32_t FINISH_GRID_NO_MIXED = 8;  // k_finish blocks when batches have no non-uniform group (launch_chunk)
 
 struct PipeSlot {
   gub_req* d_req = nullptr;
@@ -61,11 +62,13 @@ struct gub_table {
   gub::Slot* table = nullptr;
   uint64_t capacity = 0;
   uint32_t max_batch = 0;
-  // per-batch scratch of the four-kernel pipeline (gub_kernels.cuh)
+  // per-batch scratch of the four-kernel pipeline (gub_kernels.cuh).  What k_group writes comes in two sets, picked by epoch parity, so
+  // that the next batch's k_group can run while the current batch still reads its set; a ring shard's table has set 0 only.
   struct Scratch {
-    gub::AuxEntry* aux = nullptr;
-    uint32_t *ent = nullptr, *meta = nullptr, *rank = nullptr, *order = nullptr, *mixed_ent = nullptr, *presence = nullptr;
-    uint8_t* fragsize = nullptr;
+    gub::AuxEntry* aux[2] = {};
+    uint32_t *ent[2] = {}, *meta[2] = {}, *presence[2] = {};
+    uint8_t* fragsize[2] = {};
+    uint32_t *rank = nullptr, *order = nullptr, *mixed_ent = nullptr;
     ulonglong2* commit = nullptr;
     gub::BatchCtr* ctr = nullptr;
     uint32_t epoch = 0;
@@ -115,6 +118,8 @@ struct gub_table {
   cudaEvent_t trace_base = nullptr;
   std::vector<cudaEvent_t> trace_ev;  // 6 per traced submission
   bool prof = false;
+  uint32_t* h_mixed_hint = nullptr;   // host-mapped word: non-uniform groups of the last batch k_eval saw (BatchArgs::mixed_hint)
+  uint32_t* d_mixed_hint = nullptr;
   std::vector<cudaEvent_t> prof_ev;   // 5 events per pending chunk
   size_t prof_pending = 0;            // chunks recorded and not yet accumulated
   double prof_ms[4] = {0, 0, 0, 0};
@@ -230,9 +235,9 @@ int launch_chunk(gub_table* t, const gub_req* d_reqs, uint32_t n, const gub_cloc
                  const uint32_t* n_dev = nullptr, uint32_t n_off = 0, const SegDesc* seg = nullptr) {
   gub_table::Scratch& sc = t->scr;
   bool wrapped = false;
-  if (sc.epoch >= 65535u) {  // 16-bit epoch tags wrapped: clear the grouping table so stale tags cannot alias
+  if (sc.epoch >= 65535u) {  // 16-bit epoch tags wrapped: clear the grouping tables so stale tags cannot alias
     wrapped = true;
-    CK(cudaMemsetAsync(sc.aux, 0, (size_t)t->aux_entries * sizeof(gub::AuxEntry), st));
+    for (gub::AuxEntry* aux : sc.aux) if (aux) CK(cudaMemsetAsync(aux, 0, (size_t)t->aux_entries * sizeof(gub::AuxEntry), st));
     // 65535 -> 1 keeps the parity: the batch after the wrap reuses ctr[1], which k_rank (it only resets the OTHER parity) left
     // holding batch 65535's allocators.  Clear both.
     CK(cudaMemsetAsync(sc.ctr, 0, 2 * sizeof(gub::BatchCtr), st));
@@ -246,11 +251,16 @@ int launch_chunk(gub_table* t, const gub_req* d_reqs, uint32_t n, const gub_cloc
     for (uint32_t k = 0; k < seg->nseg; k++) { A.seg_reqs[k] = seg->reqs[k]; A.seg_out[k] = seg->out[k]; }
   }
   A.table = t->table; A.capacity = t->capacity; A.reqs = d_reqs; A.out = d_out; A.n = n; A.n_dev = n_dev; A.n_off = n_off; A.epoch = sc.epoch;
-  A.aux = sc.aux; A.aux_mask = t->aux_entries - 1; A.presence = sc.presence; A.fragsize = sc.fragsize;
-  A.pres_words = t->pres_words; A.max_blocks = t->max_blocks; A.ent = sc.ent; A.meta = sc.meta; A.rank = sc.rank;
+  const bool two_sets = sc.aux[1] != nullptr;
+  const uint32_t par = two_sets ? (sc.epoch & 1u) : 0u;
+  A.aux = sc.aux[par]; A.aux_mask = t->aux_entries - 1; A.presence = sc.presence[par]; A.fragsize = sc.fragsize[par];
+  A.pres_words = t->pres_words; A.max_blocks = t->max_blocks; A.ent = sc.ent[par]; A.meta = sc.meta[par]; A.rank = sc.rank;
   A.commit = sc.commit; A.order = sc.order; A.mixed_ent = sc.mixed_ent; A.ctr = sc.ctr;
   A.counters = t->counters; A.ovf = t->ovf; A.ovf_count = &t->ctl->ovf_count; A.inv = t->inv;
   A.ktrace = t->ktrace;
+  A.chain_done = &t->ctl->chain_done;
+  A.early_ok = (two_sets && sc.epoch > 1u) ? 1u : 0u;  // (epoch 1: the first batch since the scratch was made or wrapped)
+  A.mixed_hint = seg ? nullptr : t->d_mixed_hint;
   A.clk = *clk;
   const uint32_t blocks = (n + 255) / 256;
   cudaEvent_t* pe = nullptr;
@@ -263,7 +273,13 @@ int launch_chunk(gub_table* t, const gub_req* d_reqs, uint32_t n, const gub_cloc
     t->prof_pending++;
     CK(cudaEventRecord(pe[0], st));
   }
-  const uint32_t fin_blocks = std::min<uint32_t>((uint32_t)t->num_sms, std::max<uint32_t>(1u, n / 2));
+  // k_finish: one block per SM, except on a single table with two scratch sets when the last batch k_eval has seen had no non-uniform
+  // group (the bench workload: every repeated key a uniform run).  Then the next batch's k_group, which launches only once every
+  // k_finish block has been resident, should not wait for 132 of them: a k_finish block (128 registers x 256 threads) fits on an SM only
+  // beside ONE k_eval block, and 65 536 requests are 256 k_eval blocks on 132 SMs x 2, so 8 fit at once.  The count read here may be a
+  // few batches old; the grid size changes how fast the non-uniform groups are worked off, never the results.
+  const bool few_mixed = !seg && two_sets && t->h_mixed_hint && *(volatile const uint32_t*)t->h_mixed_hint == 0;
+  const uint32_t fin_blocks = std::min<uint32_t>(few_mixed ? FINISH_GRID_NO_MIXED : (uint32_t)t->num_sms, std::max<uint32_t>(1u, n / 2));
   if (seg) {
     CK(launch_k(t, gub::k_group<true>, blocks, gub::GROUP_THREADS, st, A, wrapped));
     if (pe) CK(cudaEventRecord(pe[1], st));
@@ -377,12 +393,22 @@ gub_item from_dev(const gub::DevItem& d) {
   return it;
 }
 
-// Per-batch scratch of the four-kernel pipeline for batches of up to B requests (replaces what was there: the device must be idle).
-int alloc_scratch(gub_table* t, uint32_t B) {
-  auto& sc = t->scr;
-  void* old[] = {sc.aux, sc.ent, sc.meta, sc.rank, sc.order, sc.mixed_ent, sc.presence, sc.fragsize, sc.commit, sc.ctr};
-  for (void* p : old) if (p) cudaFree(p);
+void free_scratch(gub_table::Scratch& sc) {
+  for (int s = 0; s < 2; s++) {
+    void* set[] = {sc.aux[s], sc.ent[s], sc.meta[s], sc.presence[s], sc.fragsize[s]};
+    for (void* p : set) if (p) cudaFree(p);
+  }
+  void* rest[] = {sc.rank, sc.order, sc.mixed_ent, sc.commit, sc.ctr};
+  for (void* p : rest) if (p) cudaFree(p);
   sc = gub_table::Scratch();
+}
+
+// Per-batch scratch of the four-kernel pipeline for batches of up to B requests (replaces what was there: the device must be idle).
+// sets = 2: a second set of what k_group writes (aux, presence, fragsize, ent, meta; 80.5 MiB more at B = 65 536), which lets the next
+// batch's k_group overlap the current batch (launch_chunk).
+int alloc_scratch(gub_table* t, uint32_t B, int sets) {
+  auto& sc = t->scr;
+  free_scratch(sc);
   B = std::max<uint32_t>(1024u, std::min<uint32_t>(B, 262144u));
   B = (B + 255u) & ~255u;
   t->max_batch = B;
@@ -390,14 +416,20 @@ int alloc_scratch(gub_table* t, uint32_t B) {
   t->max_blocks = (B / gub::GROUP_THREADS + 127u) & ~127u;  // fragment-size row per group entry; a multiple of 128 blocks = 4 presence words (16-byte loads)
   t->pres_words = t->max_blocks / 32;
   struct { void** p; size_t bytes; } want[] = {
-      {(void**)&sc.aux, (size_t)t->aux_entries * sizeof(gub::AuxEntry)},
-      {(void**)&sc.presence, (size_t)t->aux_entries * t->pres_words * 4},
-      {(void**)&sc.fragsize, (size_t)t->aux_entries * t->max_blocks},
+      {(void**)&sc.aux[0], (size_t)t->aux_entries * sizeof(gub::AuxEntry)},
+      {(void**)&sc.presence[0], (size_t)t->aux_entries * t->pres_words * 4},
+      {(void**)&sc.fragsize[0], (size_t)t->aux_entries * t->max_blocks},
+      {(void**)&sc.ent[0], (size_t)B * 4}, {(void**)&sc.meta[0], (size_t)B * 4},
+      {(void**)&sc.aux[1], sets > 1 ? (size_t)t->aux_entries * sizeof(gub::AuxEntry) : 0},
+      {(void**)&sc.presence[1], sets > 1 ? (size_t)t->aux_entries * t->pres_words * 4 : 0},
+      {(void**)&sc.fragsize[1], sets > 1 ? (size_t)t->aux_entries * t->max_blocks : 0},
+      {(void**)&sc.ent[1], sets > 1 ? (size_t)B * 4 : 0}, {(void**)&sc.meta[1], sets > 1 ? (size_t)B * 4 : 0},
       {(void**)&sc.commit, (size_t)t->aux_entries * 6 * sizeof(ulonglong2)},
-      {(void**)&sc.ent, (size_t)B * 4}, {(void**)&sc.meta, (size_t)B * 4}, {(void**)&sc.rank, (size_t)B * 4}, {(void**)&sc.order, (size_t)B * 4},
+      {(void**)&sc.rank, (size_t)B * 4}, {(void**)&sc.order, (size_t)B * 4},
       {(void**)&sc.mixed_ent, ((size_t)B / 2 + 1) * 4}, {(void**)&sc.ctr, 2 * sizeof(gub::BatchCtr)},
   };
   for (auto& w : want) {
+    if (!w.bytes) continue;
     cudaError_t e = cudaMalloc(w.p, w.bytes);
     if (e != cudaSuccess) return fail(std::string("cudaMalloc(batch scratch): ") + cudaGetErrorString(e));
     CK(cudaMemset(*w.p, 0, w.bytes));
@@ -420,11 +452,7 @@ void gub_destroy(gub_table* t) {
   void* ptrs[] = {t->table, t->counters, t->d_scalar, t->d_ring_pts, t->d_ring_peers, t->d_ring_lut, t->d_owner, t->d_tile_counts,
                   t->gaux, t->gpres, t->gfrag, t->gmembers, t->ctl, t->ovf, t->trace, t->ktrace, t->inv.e};
   for (void* p : ptrs) if (p) cudaFree(p);
-  {
-    auto& sc = t->scr;
-    void* sp[] = {sc.aux, sc.ent, sc.meta, sc.rank, sc.order, sc.mixed_ent, sc.presence, sc.fragsize, sc.commit, sc.ctr};
-    for (void* p : sp) if (p) cudaFree(p);
-  }
+  free_scratch(t->scr);
   for (auto& s : t->pipe) {
     if (s.d_req) cudaFree(s.d_req);
     if (s.d_resp) cudaFree(s.d_resp);
@@ -436,6 +464,7 @@ void gub_destroy(gub_table* t) {
   }
   for (auto& e : t->compute_done) if (e) cudaEventDestroy(e);
   for (auto& e : t->prof_ev) cudaEventDestroy(e);
+  if (t->h_mixed_hint) cudaFreeHost(t->h_mixed_hint);
   if (t->last_done) cudaEventDestroy(t->last_done);
   if (t->s_h2d) cudaStreamDestroy(t->s_h2d);
   if (t->s_compute) cudaStreamDestroy(t->s_compute);
@@ -473,7 +502,8 @@ int gub_create(const gub_config* cfg, gub_table** out) {
     cudaMemset((ptr), 0, (bytes));                                           \
   } while (0)
   ALLOC(t->table, t->capacity * sizeof(gub::Slot));
-  if (alloc_scratch(t, t->max_batch)) { gub_destroy(t); return -1; }
+  // two scratch sets up to 65 536 requests per batch (80.5 MiB more); beyond that the second set would cost 4 x as much per 4 x requests
+  if (alloc_scratch(t, t->max_batch, t->max_batch <= 65536u ? 2 : 1)) { gub_destroy(t); return -1; }
   t->num_sms = std::min<int>(prop.multiProcessorCount, gub::FB_MAX_GRID);
   if (const char* e = getenv("GUB_PATH")) t->fused = std::string(e) == "fused";
   if (const char* e = getenv("GUB_COOP")) t->coop = std::atoi(e) != 0;
@@ -484,6 +514,11 @@ int gub_create(const gub_config* cfg, gub_table** out) {
   ALLOC(t->ctl, sizeof(gub::FCtl));
   ALLOC(t->ovf, (size_t)gub::FB_OVF_CAP * sizeof(gub::OvfItem));
   ALLOC(t->inv.e, (size_t)65536 * sizeof(gub::InvEntry));
+  {
+    cudaError_t e = cudaHostAlloc((void**)&t->h_mixed_hint, sizeof(uint32_t), cudaHostAllocMapped);
+    if (e == cudaSuccess) { *t->h_mixed_hint = 0; e = cudaHostGetDevicePointer((void**)&t->d_mixed_hint, t->h_mixed_hint, 0); }
+    if (e != cudaSuccess) { fail(std::string("cudaHostAlloc(mixed_hint): ") + cudaGetErrorString(e)); gub_destroy(t); return -1; }
+  }
   t->inv.mask = 65535;
   {
     // incremental expiry sweep: the whole table once every ~65536 batches (GUB_SWEEP=<slots per CTA per batch>, 0 = off)
@@ -1312,7 +1347,7 @@ int gub_p2p_create(gub_table* t, const gub_ring* ring, uint32_t rank, uint32_t c
     std::lock_guard<std::mutex> lk(t->mu);
     if (t->max_batch < want) {
       CK(cudaDeviceSynchronize());
-      if (alloc_scratch(t, want)) return -1;
+      if (alloc_scratch(t, want, 1)) return -1;  // a ring shard's batches wait for their k_seg_wait: one set
     }
   }
   gub_p2p* p = new gub_p2p();

@@ -66,7 +66,7 @@ struct FSeg {                           // one run of request records, evaluated
 
 struct FCtl {
   uint32_t bar_cnt, bar_gen;            // grid barrier
-  uint32_t _spare;
+  uint32_t chain_done;                  // four-kernel pipeline: epoch of the last batch whose k_finish has finished (BatchArgs::chain_done)
   uint32_t done_ctr;                    // CTAs that have stored all their responses (multi-GPU: the last one publishes the flags)
   uint32_t error;                       // a flag wait timed out (a peer died)
   uint32_t ovf_count;                   // pending items in `ovf`
@@ -121,8 +121,6 @@ struct MBar { uint64_t w; };
 __device__ __forceinline__ void mbar_init(MBar*) {}
 __device__ __forceinline__ void tile_load(void* dst, const void* src, uint32_t bytes, MBar*) { std::memcpy(dst, src, bytes); }
 __device__ __forceinline__ void mbar_wait(MBar*, uint32_t) {}
-__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) { return *p; }
-__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) { *p = v; }
 __device__ __forceinline__ void spin_pause() { emu::spin_yield(); }
 __device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t* p) { return *p; }
 __device__ __forceinline__ void st_relaxed_gpu(uint32_t* p, uint32_t v) { *p = v; }
@@ -152,12 +150,6 @@ __device__ __forceinline__ void mbar_wait(MBar* b, uint32_t parity) {
                  : "memory");
   }
 }
-__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ void spin_pause() {}
 __device__ __forceinline__ uint32_t ld_relaxed_gpu(const uint32_t* p) {
   uint32_t v;

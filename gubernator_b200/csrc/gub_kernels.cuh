@@ -108,6 +108,11 @@ struct BatchArgs {
   const gub_req* seg_reqs[MAX_SHARDS];
   gub_resp* seg_out[MAX_SHARDS];
   unsigned long long* ktrace;  // optional (diagnostic, gub_set_trace): [4 kernels][KT_BLOCKS][KT_MARKS] latest %globaltimer at which a warp / a thread in a role passed a mark
+  // Early hand-off (single table, see k_group): *chain_done = epoch of the last batch whose k_finish block 0 has left (it stores the
+  // epoch last); early_ok = this batch's grouping scratch is not the previous batch's (two scratch sets) and epoch > 1.  chain_done may be null.
+  uint32_t* chain_done;
+  uint32_t early_ok;
+  uint32_t* mixed_hint;    // optional, host-mapped: k_eval copies the batch's count of non-uniform groups here (sizes later k_finish grids)
   gub_clock clk;
 };
 constexpr int KT_MARKS = 8, KT_BLOCKS = 1024;
@@ -153,12 +158,20 @@ __device__ __forceinline__ void kt_stamp(unsigned long long* ktrace, int kernel,
 #define KT(A, kernel, mark, dep, all) kt_stamp((A).ktrace, kernel, mark, (uint32_t)(dep), all)
 #endif
 
-// system-scope release / acquire on flags other GPUs (or the host) poll
+// system-scope release / acquire on flags other GPUs (or the host) poll; gpu-scope ones on words only this device's kernels use
 #if defined(GUB_EMULATE)
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) { *p = v; }
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long* p) { return *p; }
+__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) { *p = v; }
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) { return *p; }
 __device__ __forceinline__ void __nanosleep(unsigned) { emu::spin_yield(); }
 #else
+__device__ __forceinline__ void st_release_gpu(uint32_t* p, uint32_t v) { asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* p) {
+  uint32_t v;
+  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+  return v;
+}
 __device__ __forceinline__ void st_release_sys(unsigned long long* p, unsigned long long v) {
   asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
@@ -528,8 +541,32 @@ __device__ void merge_colliding_fragments(const BatchArgs& A, const uint32_t* s_
   if (valid && s_tlocal[threadIdx.x] != 0xFFFFu) { local = s_tlocal[threadIdx.x]; sp = s_tsp[threadIdx.x]; }
 }
 
+// What k_group does right after its wait.  Inserts a previous batch could not place (probe window full) are placed now, with eviction:
+// the previous batch is complete and this batch's k_rank has not passed its wait (it waits for this grid), so nothing can observe a
+// half-moved entry.
+__device__ __forceinline__ void group_waited(const BatchArgs& A) {
+  KT(A, 0, KT_WAITED, 0, false);
+  if (blockIdx.x == 0 && threadIdx.x < 32 && __ldcg(A.ovf_count)) {
+    uint32_t ins = 0;
+    drain_parked(A.table, A.capacity, A.ovf, A.ovf_count, A.clk.now_ms, A.counters, &ins);
+    if (threadIdx.x == 0 && ins) atomicAdd(A.counters + C_INSERTS, (unsigned long long)ins);
+  }
+}
+
+// Early hand-off (single table): apart from that drain k_group does not touch the table, and it writes only the grouping scratch of its
+// epoch's parity, which the batch before it does not use, so its body need not wait for that batch.  It does read the request records, which PDL guarantees only
+// after the wait.  A block therefore looks at *chain_done first:
+//  - it is not the previous epoch: k_finish of the previous batch has not finished, so this launch started as ITS programmatic
+//    dependent.  A plain kernel in between would have waited for that k_finish to complete, and a memory operation breaks the
+//    programmatic edge altogether, so nothing ran between the two submissions: the records were complete before the previous batch's
+//    chain began (its k_rank waited for its k_group, which waited for everything earlier).  The block triggers its dependents, does its
+//    whole body, and waits before it exits, so this grid's completion (what k_rank waits for) still implies the previous batch's.
+//  - it is the previous epoch, or early_ok is off (first batch, one scratch set, ring mode): wait first, as before.
+// Not detected: a caller kernel launched programmatically between two submissions that triggers its dependents before its last write of
+// the records.  Blocks decide independently; either choice is correct for a block.
 template <bool SEG>
 __global__ void __launch_bounds__(GROUP_THREADS) k_group(const BatchArgs A) {
+  __shared__ uint32_t s_early;
   __shared__ unsigned long long s_key[GROUP_SLOTS];
   __shared__ uint32_t s_cnt[GROUP_SLOTS];  // members of the key in this block
   __shared__ uint32_t s_pos[GROUP_SLOTS];  // batch-wide entry position
@@ -543,22 +580,25 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_group(const BatchArgs A) {
   if (threadIdx.x == 0) s_conflict = 0u;
   reinterpret_cast<uint4*>(&s_wcnt[0][0])[threadIdx.x] = make_uint4(0u, 0u, 0u, 0u);
   KT(A, 0, KT_ENTRY, 0, false);
-  pdl_wait();
-  pdl_release();
-  KT(A, 0, KT_WAITED, 0, false);
+  if (threadIdx.x == 0) s_early = (!SEG && A.early_ok && ld_acquire_gpu(A.chain_done) != A.epoch - 1u) ? 1u : 0u;
+  __syncthreads();
+  const bool early = s_early != 0;
+  if (early) {
+    pdl_release();
+  } else {
+    pdl_wait();
+    pdl_release();
+    group_waited(A);
+  }
   const Io<SEG> io = io_open<SEG>(A);
   __syncthreads();
-  // Inserts a previous batch could not place (probe window full) are placed now, with eviction: this kernel never reads the table
-  // and the previous batch is complete, so nothing can observe a half-moved entry.
-  if (blockIdx.x == 0 && threadIdx.x < 32 && __ldcg(A.ovf_count)) {
-    uint32_t ins = 0;
-    drain_parked(A.table, A.capacity, A.ovf, A.ovf_count, A.clk.now_ms, A.counters, &ins);
-    if (threadIdx.x == 0 && ins) atomicAdd(A.counters + C_INSERTS, (unsigned long long)ins);
-  }
   const uint32_t i = blockIdx.x * GROUP_THREADS + threadIdx.x;
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const uint32_t n = batch_n(A);  // after the wait: an earlier kernel may have just written it
-  if (blockIdx.x * GROUP_THREADS >= n) return;  // whole block beyond the batch (uniform: no barrier is skipped by part of a block)
+  const uint32_t n = batch_n(A);  // an earlier kernel may have written it: after the wait, or (early) complete like the records
+  if (blockIdx.x * GROUP_THREADS >= n) {  // whole block beyond the batch (uniform: no barrier is skipped by part of a block)
+    if (early) { pdl_wait(); group_waited(A); }
+    return;
+  }
   const bool valid = i < n;
   uint32_t sp = 0xFFFFu;  // shared-memory slot of my key (0xFFFF: no request)
   uint64_t key = 0;
@@ -613,6 +653,10 @@ __global__ void __launch_bounds__(GROUP_THREADS) k_group(const BatchArgs A) {
   if (valid) {
     A.ent[i] = s_pos[sp];
     A.meta[i] = (sp << 16) | local;
+  }
+  if (early) {
+    pdl_wait();
+    group_waited(A);
   }
   KT(A, 0, KT_EXIT, 0, false);
 }
@@ -815,6 +859,7 @@ __global__ void __launch_bounds__(GROUP_THREADS, 2) k_eval(const BatchArgs A) {
   pdl_wait();
   pdl_release();
   KT(A, 2, KT_WAITED, 0, false);
+  if (A.mixed_hint && blockIdx.x == 0 && threadIdx.x == 0) *(volatile uint32_t*)A.mixed_hint = __ldcg(&A.ctr[A.epoch & 1].n_mixed);  // final: k_rank is complete
   if (i < n) {
     const uint32_t pos = A.ent[i];
     const uint32_t rank = A.rank[i];             // garbage for keys seen once: not used
@@ -1048,6 +1093,13 @@ __device__ void mixed_group(const BatchArgs& A, const Io<SEG>& io, uint32_t pos,
 }
 
 // Non-uniform groups, one block each (grid-stride).  A launch with nothing to finish — the usual case — returns at once.
+// Single table: it triggers its dependents at entry, so that the next batch's k_group can start beside this batch's tail.  That k_group
+// launches only once every k_finish block has been resident, and a k_finish block (128 registers x 256 threads) fits on an SM only beside
+// one k_eval block, so blocks that will find no group leave before the wait and hand their place on: the number of non-uniform groups was
+// written by k_rank, which completed before k_eval passed its wait, i.e. two kernels ago (safe ahead of the wait, like batch_n in
+// k_rank).  A stale read would only leave more of the queue to the blocks that stay.  Block 0 always waits (a grid whose blocks all
+// skipped the wait would complete before its predecessor and break the chain of waits) and, last, stores the epoch into *chain_done: until
+// then the next batch's k_group knows this grid has not finished (see k_group).
 template <bool SEG>
 #if !defined(GUB_FINISH_MIN_BLOCKS)
 #define GUB_FINISH_MIN_BLOCKS 2  // 128 registers (the segment fold spills a little): an empty k_finish block must fit next to a k_eval / k_rank block
@@ -1056,27 +1108,38 @@ __global__ void __launch_bounds__(MIXED_THREADS, GUB_FINISH_MIN_BLOCKS) k_finish
   __shared__ MixedShared S;
   Tally t = {0, 0, 0, 0, 0};
   KT(A, 3, KT_ENTRY, 0, false);
+  if constexpr (!SEG) {
+    pdl_release();
+    if (blockIdx.x != 0) {
+      __shared__ uint32_t s_idle;
+      if (threadIdx.x == 0) s_idle = blockIdx.x >= __ldcg(&A.ctr[A.epoch & 1].n_mixed) ? 1u : 0u;
+      __syncthreads();
+      if (s_idle) return;
+    }
+  }
   pdl_wait();
-  pdl_release();
+  if constexpr (SEG) pdl_release();
   KT(A, 3, KT_WAITED, 0, false);
   const BatchCtr ctr = A.ctr[A.epoch & 1];
-  if (ctr.n_mixed == 0) return;
-  const Io<SEG> io = io_open<SEG>(A);
-  // groups differ a lot in size (a hot key's group has thousands of members): blocks pull the next one when they are done
-  __shared__ uint32_t s_next;
-  for (;;) {
-    if (threadIdx.x == 0) s_next = atomicAdd(&A.ctr[A.epoch & 1].next_mixed, 1u);
-    __syncthreads();
-    const uint32_t g = s_next;
-    if (g >= ctr.n_mixed) break;
-    mixed_group(A, io, A.mixed_ent[g], S, t);
-    __syncthreads();
+  if (ctr.n_mixed != 0) {
+    const Io<SEG> io = io_open<SEG>(A);
+    // groups differ a lot in size (a hot key's group has thousands of members): blocks pull the next one when they are done
+    __shared__ uint32_t s_next;
+    for (;;) {
+      if (threadIdx.x == 0) s_next = atomicAdd(&A.ctr[A.epoch & 1].next_mixed, 1u);
+      __syncthreads();
+      const uint32_t g = s_next;
+      if (g >= ctr.n_mixed) break;
+      mixed_group(A, io, A.mixed_ent[g], S, t);
+      __syncthreads();
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+      atomicAdd(A.counters + C_DUP_GROUPS, (unsigned long long)ctr.n_mixed);
+      atomicAdd(A.counters + C_MIXED_GROUPS, (unsigned long long)ctr.n_mixed);
+    }
+    tally_flush_block(t, A.counters);
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    atomicAdd(A.counters + C_DUP_GROUPS, (unsigned long long)ctr.n_mixed);
-    atomicAdd(A.counters + C_MIXED_GROUPS, (unsigned long long)ctr.n_mixed);
-  }
-  tally_flush_block(t, A.counters);
+  if (blockIdx.x == 0 && threadIdx.x == 0 && A.chain_done) st_release_gpu(A.chain_done, A.epoch);
 }
 
 // ---- key hashing on the device: client.go:39-41 HashKey + workers.go:153 XXH64 + replicated_hash.go:108 FNV-1 ----------

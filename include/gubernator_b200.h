@@ -128,7 +128,9 @@ typedef struct {
 
 typedef struct {
   uint64_t capacity_slots; /* table size in 64-byte slots (>= 2x expected live keys); replaces Config.CacheSize (config.go:86) */
-  uint32_t max_batch;      /* largest batch evaluated by one launch sequence; larger submits are chunked in order. 0 = 65536 */
+  uint32_t max_batch;      /* largest batch evaluated by one launch sequence; larger submits are chunked in order. 0 = 65536.
+                              Up to 65 536 the table keeps two sets of grouping scratch (80.5 MiB more at 65 536) so that
+                              consecutive batches on one stream overlap (see gub_submit_device). */
   int32_t device;          /* CUDA device ordinal */
 } gub_config;
 
@@ -143,7 +145,12 @@ int gub_abi_version(void);
 /* ---- the hot path: WorkerPool.GetRateLimit (workers.go:261-324) for a whole batch -------------------------- */
 /* Host buffers: copies requests H2D, evaluates, copies responses D2H, returns when `out` is filled. */
 int gub_submit(gub_table* t, const gub_req* reqs, size_t n, const gub_clock* clk, gub_resp* out);
-/* Device buffers (already resident in this GPU's HBM); enqueued on `stream` (a cudaStream_t), returns immediately. */
+/* Device buffers (already resident in this GPU's HBM); enqueued on `stream` (a cudaStream_t), returns immediately.
+ * When two submissions follow each other on one stream with nothing in between, the second one's grouping kernel reads its
+ * requests while the first one is still evaluated (programmatic dependent launch).  A kernel the caller puts in between is
+ * detected on the device and makes the second submission wait for it; the one case that is not detected is a caller kernel
+ * launched with programmatic stream serialization that triggers its dependents (griddepcontrol.launch_dependents) before its
+ * last write of the requests.  Plain kernels, copies and event waits in between are safe. */
 int gub_submit_device(gub_table* t, const gub_req* d_reqs, size_t n, const gub_clock* clk, gub_resp* d_out, void* stream);
 /* Same, when the batch size is only known on the device: *d_n (<= n_cap) requests; launches are sized for n_cap. */
 int gub_submit_device_n(gub_table* t, const gub_req* d_reqs, size_t n_cap, const uint32_t* d_n, const gub_clock* clk, gub_resp* d_out, void* stream);
