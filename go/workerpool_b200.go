@@ -18,11 +18,13 @@ package gubernator
 #cgo LDFLAGS: -lgubernator_b200
 #include <stdlib.h>
 #include "gubernator_b200.h"
+extern int b200StoreGet(void* user, gub_store_rec* misses, size_t n);
 */
 import "C"
 
 import (
 	"context"
+	"runtime/cgo"
 	"sync"
 	"time"
 	"unsafe"
@@ -49,6 +51,8 @@ type B200WorkerPool struct {
 	packed    unsafe.Pointer
 	packedCap int
 	resps     unsafe.Pointer
+	// with a conf.Store: the change log the device writes (gub_submit_keys_store_async), pinned
+	changes, nChanges unsafe.Pointer
 	overLimit uint64 // last gub_counters.over_limit seen: the metric is fed from the device's own count
 	// key strings by fingerprint, kept only when a Loader needs CacheItem.Key back (store.go:69-78)
 	mu   sync.Mutex
@@ -72,12 +76,6 @@ const (
 )
 
 func NewB200WorkerPool(conf *Config) (*B200WorkerPool, error) {
-	if conf.Store != nil {
-		// Store.Get / OnChange / Remove are honoured at batch granularity by the C++ host layer (gub_instance_set_store,
-		// include/gubernator_b200_host.h); this shim does not route them through cgo callbacks, and silently ignoring a
-		// configured Store would lose data.
-		return nil, errors.New("B200WorkerPool: conf.Store is not supported by the cgo shim (use a Loader, or the C++ host layer)")
-	}
 	cfg := C.gub_config{
 		capacity_slots: C.uint64_t(2 * conf.CacheSize), // load factor <= 0.5; replaces CacheSize/Workers LRUs (workers.go:132)
 		max_batch:      b200MaxBatch,
@@ -90,6 +88,10 @@ func NewB200WorkerPool(conf *Config) (*B200WorkerPool, error) {
 	p.packedCap = b200MaxBatch*(16+4+b200KeyBytes) + 64
 	p.packed = C.gub_host_alloc(C.size_t(p.packedCap))
 	p.resps = C.gub_host_alloc(C.size_t(b200MaxBatch * 32))
+	if conf.Store != nil {
+		p.changes = C.gub_host_alloc(C.size_t(b200MaxBatch * C.sizeof_gub_store_rec))
+		p.nChanges = C.gub_host_alloc(4)
+	}
 	if conf.Loader != nil {
 		p.keys = make(map[[2]uint64]string)
 	}
@@ -211,9 +213,32 @@ func (p *B200WorkerPool) flush(batch []*pendingReq) {
 	var clk C.gub_clock
 	C.gub_clock_fill(C.int64_t(clock.Now().UnixNano()/1000000), &clk)
 	var ticket C.int
-	rc := C.gub_submit_keys_async(p.table, p.packed, total, C.size_t(n), &params[0], C.size_t(len(params)), C.int64_t(base), &clk, &resps[0], &ticket)
+	var rc C.int
+	if p.conf.Store == nil {
+		rc = C.gub_submit_keys_async(p.table, p.packed, total, C.size_t(n), &params[0], C.size_t(len(params)), C.int64_t(base), &clk, &resps[0], &ticket)
+	} else {
+		// Store.Get runs inside the call (b200StoreGet, once per batch, for its misses); Remove / OnChange are replayed below
+		h := cgo.NewHandle(&storeCall{p: p, batch: batch, keys: keys})
+		rc = C.gub_submit_keys_store_async(p.table, p.packed, total, C.size_t(n), &params[0], C.size_t(len(params)), C.int64_t(base), &clk,
+			C.gub_store_get_fn(C.b200StoreGet), unsafe.Pointer(&h), &resps[0], (*C.gub_store_rec)(p.changes), (*C.uint32_t)(p.nChanges), &ticket)
+		h.Delete()
+	}
 	if rc == 0 {
 		rc = C.gub_wait(p.table, ticket)
+	}
+	if rc == 0 && p.conf.Store != nil {
+		// one record per key, ordered by its first request: Remove, then OnChange, as the reference calls them (algorithms.go)
+		ctx := context.Background()
+		for _, r := range unsafe.Slice((*C.gub_store_rec)(p.changes), int(*(*C.uint32_t)(p.nChanges))) {
+			if r.flags&C.GUB_STORE_REMOVE != 0 {
+				p.conf.Store.Remove(ctx, keys[r.first])
+			}
+			if r.flags&C.GUB_STORE_CHANGE != 0 {
+				item := p.fromItem(&r.item)
+				item.Key = keys[r.first]
+				p.conf.Store.OnChange(ctx, batch[r.last].req, item)
+			}
+		}
 	}
 	for i, pr := range batch {
 		if rc != 0 {
@@ -238,6 +263,34 @@ func (p *B200WorkerPool) flush(batch []*pendingReq) {
 		}
 		p.overLimit = uint64(c.over_limit)
 	}
+}
+
+type storeCall struct {
+	p     *B200WorkerPool
+	batch []*pendingReq
+	keys  []string
+}
+
+// b200StoreGet is the batch's Store.Get (algorithms.go:45-51): one call per key that missed, with the key's first request.
+//
+//export b200StoreGet
+func b200StoreGet(user unsafe.Pointer, misses *C.gub_store_rec, n C.size_t) C.int {
+	sc := (*(*cgo.Handle)(user)).Value().(*storeCall)
+	ms := unsafe.Slice(misses, int(n))
+	for i := range ms {
+		m := &ms[i]
+		item, ok := sc.p.conf.Store.Get(context.Background(), sc.batch[m.first].req)
+		if !ok || item == nil {
+			continue
+		}
+		it, known := toItem(sc.keys[m.first], item)
+		if !known {
+			it.algorithm = -1 // a Value the cache cannot hold: counted as existing, never installed
+		}
+		m.item = it
+		m.flags |= C.GUB_STORE_FOUND
+	}
+	return 0
 }
 
 // b200Error rebuilds the error values handleGetRateLimit returns (workers.go:299-320); V1Instance wraps them further.
@@ -386,6 +439,8 @@ func (p *B200WorkerPool) Close() error {
 	p.done.Wait()
 	C.gub_host_free(p.packed)
 	C.gub_host_free(p.resps)
+	C.gub_host_free(p.changes)
+	C.gub_host_free(p.nChanges)
 	C.gub_destroy(p.table)
 	return nil
 }

@@ -21,6 +21,7 @@
 #include "gub_batch.cuh"
 #include "gub_global.cuh"
 #include "gub_p2p.cuh"
+#include "gub_store.cuh"
 
 extern "C" uint64_t gub_ring_version_(const gub_ring* r);
 
@@ -124,6 +125,21 @@ struct gub_table {
   size_t prof_pending = 0;            // chunks recorded and not yet accumulated
   double prof_ms[4] = {0, 0, 0, 0};
   uint64_t prof_launches = 0;
+  // the Store plugin's pre- and post-pass (gub_store.cuh, gub_submit_keys_store_async), allocated on first use, sized for max_batch
+  struct StoreScratch {
+    gub::StoreKey* keys = nullptr;
+    uint32_t key_entries = 0, epoch = 0;
+    uint32_t *kent = nullptr, *blk = nullptr, *d_failed = nullptr;
+    gub::StoreState* bstate = nullptr;
+    uint8_t* sel = nullptr;
+    gub_store_rec* sparse = nullptr;
+    // page-locked, read by the device in place: the miss list the Get callback receives, its count, the verdicts and items to install
+    gub_store_rec* h_miss = nullptr;
+    uint32_t* h_count = nullptr;
+    uint4* h_loaded = nullptr;
+    gub::DevItem* h_items = nullptr;
+    cudaEvent_t misses_done = nullptr;
+  } store;
 };
 
 namespace {
@@ -464,6 +480,14 @@ void gub_destroy(gub_table* t) {
   }
   for (auto& e : t->compute_done) if (e) cudaEventDestroy(e);
   for (auto& e : t->prof_ev) cudaEventDestroy(e);
+  {
+    auto& ss = t->store;
+    void* dev[] = {ss.keys, ss.kent, ss.blk, ss.d_failed, ss.bstate, ss.sel, ss.sparse};
+    for (void* p : dev) if (p) cudaFree(p);
+    void* host[] = {ss.h_miss, ss.h_count, ss.h_loaded, ss.h_items};
+    for (void* p : host) if (p) cudaFreeHost(p);
+    if (ss.misses_done) cudaEventDestroy(ss.misses_done);
+  }
   if (t->h_mixed_hint) cudaFreeHost(t->h_mixed_hint);
   if (t->last_done) cudaEventDestroy(t->last_done);
   if (t->s_h2d) cudaStreamDestroy(t->s_h2d);
@@ -656,11 +680,128 @@ int gub_keys_layout(size_t n, size_t key_bytes, size_t* offsets_at, size_t* byte
   return 0;
 }
 
-int gub_submit_keys_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params, int64_t created_base,
-                          const gub_clock* clk, gub_resp* out, int* ticket) {
-  if (!t || !clk || !ticket || (n && (!packed || !out || !params))) return fail("gub_submit_keys_async: null argument");
-  if (n > 0x7FFFFFFFull || n_params > 0xFFFFFFFFull) return fail("gub_submit_keys_async: too large");
-  if (n && packed_bytes < n * sizeof(gub_kreq) + (n + 1) * 4) return fail("gub_submit_keys_async: packed buffer too small");
+}  // extern "C"
+
+extern "C" {
+namespace {
+int drain_pending(gub_table* t, cudaStream_t st = 0);  // (defined with gub_add_items)
+}  // namespace
+}  // extern "C"
+
+namespace {
+
+// A Store plugin's part in one submission (gub_submit_keys_store_async): the Get callback and where the change log goes (device views
+// of the caller's page-locked buffers).
+struct StoreCall {
+  gub_store_get_fn get;
+  void* user;
+  gub_store_rec* changes;
+  uint32_t* n_changes;
+};
+
+int store_ensure(gub_table* t) {
+  auto& ss = t->store;
+  if (ss.keys) return 0;
+  const size_t B = t->max_batch;
+  ss.key_entries = next_pow2((uint64_t)B * 2);
+  struct { void** p; size_t bytes; } dev[] = {
+      {(void**)&ss.keys, (size_t)ss.key_entries * sizeof(gub::StoreKey)}, {(void**)&ss.kent, B * 4},
+      {(void**)&ss.blk, (B / gub::STORE_THREADS + 1) * 4}, {(void**)&ss.d_failed, 4}, {(void**)&ss.bstate, B * sizeof(gub::StoreState)},
+      {(void**)&ss.sel, B}, {(void**)&ss.sparse, B * sizeof(gub_store_rec)}};
+  for (auto& d : dev) {
+    CK(cudaMalloc(d.p, d.bytes));
+    CK(cudaMemset(*d.p, 0, d.bytes));
+  }
+  struct { void** p; size_t bytes; } host[] = {{(void**)&ss.h_miss, B * sizeof(gub_store_rec)}, {(void**)&ss.h_count, 64},
+                                               {(void**)&ss.h_loaded, B * sizeof(uint4)}, {(void**)&ss.h_items, B * sizeof(gub::DevItem)}};
+  for (auto& h : host) CK(cudaHostAlloc(h.p, h.bytes, cudaHostAllocMapped));
+  CK(cudaEventCreateWithFlags(&ss.misses_done, cudaEventDisableTiming));
+  return 0;
+}
+
+template <typename T>
+int device_view(T* host_ptr, T** dev_ptr) {
+  CK(cudaHostGetDevicePointer((void**)dev_ptr, host_ptr, 0));
+  return 0;
+}
+
+// Before the batch (host layer: gub_get_items, Store.Get, gub_add_items): the per-key dedup, the lookup of every key at its first
+// request and, with a Get callback, the miss list, the call and the installation of what the store returned.
+int store_before(gub_table* t, const gub_req* d_req, uint32_t n, const gub_clock* clk, const StoreCall& sc, gub::StoreArgs& S, cudaStream_t st) {
+  if (store_ensure(t)) return -1;
+  if (order_after_last(t, st)) return -1;  // the lookups read the table
+  auto& ss = t->store;
+  if (ss.epoch >= 0xFFFFFFFFu) {  // the epoch tags of the dedup scratch wrapped: stale entries must not alias
+    CK(cudaMemsetAsync(ss.keys, 0, (size_t)ss.key_entries * sizeof(gub::StoreKey), st));
+    ss.epoch = 0;
+  }
+  ss.epoch++;
+  std::memset(&S, 0, sizeof S);
+  S.reqs = d_req; S.n = n; S.epoch = ss.epoch; S.keys = ss.keys; S.key_mask = ss.key_entries - 1; S.kent = ss.kent; S.bstate = ss.bstate;
+  S.sel = ss.sel; S.sparse = ss.sparse; S.blk = ss.blk; S.table = t->table; S.capacity = t->capacity; S.ovf = t->ovf;
+  S.ovf_count = &t->ctl->ovf_count; S.inv = t->inv; S.now_ms = clk->now_ms; S.want_misses = sc.get ? 1u : 0u;
+  const unsigned blocks = (n + gub::STORE_THREADS - 1) / gub::STORE_THREADS;
+  gub::k_store_keys<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
+  gub::k_store_before<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
+  CK(cudaGetLastError());
+  t->last_stream = st; t->last_pending = true;
+  if (!sc.get) return 0;
+  gub_store_rec* d_miss;
+  uint32_t* d_count;
+  if (device_view(ss.h_miss, &d_miss) || device_view(ss.h_count, &d_count)) return -1;
+  gub::k_store_compact<<<blocks, gub::STORE_THREADS, 0, st>>>(ss.sel, ss.sparse, ss.blk, n, d_miss, d_count);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(ss.misses_done, st));
+  CK(cudaEventSynchronize(ss.misses_done));
+  const uint32_t m = *(volatile uint32_t*)ss.h_count;
+  if (m == 0) return 0;
+  std::vector<uint64_t> keys((size_t)m * 2);  // the callback may write the whole item; the keys are the library's
+  for (uint32_t k = 0; k < m; k++) { keys[2 * k] = ss.h_miss[k].item.key_xxh64; keys[2 * k + 1] = ss.h_miss[k].item.key_fnv1; }
+  const int rc = sc.get(sc.user, ss.h_miss, m);
+  if (rc != 0) return fail("gub_submit_keys_store_async: the store's get callback failed (" + std::to_string(rc) + "); nothing was evaluated");
+  uint32_t nl = 0, ni = 0;
+  for (uint32_t k = 0; k < m; k++) {
+    gub_store_rec& r = ss.h_miss[k];
+    if (!(r.flags & GUB_STORE_FOUND)) continue;
+    r.item.key_xxh64 = keys[2 * k]; r.item.key_fnv1 = keys[2 * k + 1];
+    // the host layer's rule for a loaded item: it existed when it had not expired; the algorithm is the one the store returned
+    ss.h_loaded[nl++] = make_uint4(r.first, r.item.expire_at >= clk->now_ms ? gub::S_EXISTED : 0u, (uint32_t)r.item.algorithm, 0u);
+    if (r.item.algorithm == GUB_TOKEN_BUCKET || r.item.algorithm == GUB_LEAKY_BUCKET) ss.h_items[ni++] = to_dev(r.item);  // as gub_add_items
+  }
+  if (nl == 0) return 0;
+  uint4* d_loaded;
+  gub::DevItem* d_items;
+  if (device_view(ss.h_loaded, &d_loaded) || device_view(ss.h_items, &d_items)) return -1;
+  if (ni) {  // what gub_add_items does: place the parked inserts, then upsert the items
+    if (drain_pending(t, st)) return -1;
+    CK(cudaMemsetAsync(ss.d_failed, 0, 4, st));
+    gub::k_add_items<<<(ni + 255) / 256, 256, 0, st>>>(t->table, t->capacity, d_items, ni, t->counters, ss.d_failed, t->inv);
+  }
+  gub::k_store_loaded<<<(nl + gub::STORE_THREADS - 1) / gub::STORE_THREADS, gub::STORE_THREADS, 0, st>>>(d_loaded, nl, ss.bstate);
+  CK(cudaGetLastError());
+  if (ni) {
+    uint32_t failed = 0;
+    CK(cudaMemcpyAsync(&failed, ss.d_failed, 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (failed) return fail("gub_submit_keys_store_async: table full for " + std::to_string(failed) + " items the store returned");
+  }
+  return 0;
+}
+
+// After the batch (host layer: the second gub_get_items, Store.Remove / Store.OnChange): the records, straight into the caller's buffers.
+int store_after(gub_table* t, const gub_resp* d_out, const StoreCall& sc, gub::StoreArgs& S, cudaStream_t st) {
+  S.out = d_out;
+  const unsigned blocks = (S.n + gub::STORE_THREADS - 1) / gub::STORE_THREADS;
+  gub::k_store_after<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
+  gub::k_store_compact<<<blocks, gub::STORE_THREADS, 0, st>>>(S.sel, S.sparse, S.blk, S.n, sc.changes, sc.n_changes);
+  CK(cudaGetLastError());
+  t->last_stream = st; t->last_pending = true;
+  return 0;
+}
+
+// gub_submit_keys_async, and with `sc` the Store's pre- and post-pass around the batch.
+int submit_keys(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params,
+                int64_t created_base, const gub_clock* clk, gub_resp* out, int* ticket, const StoreCall* sc) {
   std::lock_guard<std::mutex> lk(t->mu);
   CK(cudaSetDevice(t->device));
   const int si = t->next_slot;
@@ -691,13 +832,54 @@ int gub_submit_keys_async(gub_table* t, const void* packed, size_t packed_bytes,
   std::memset(&P, 0, sizeof P);
   if (inl) std::memcpy(&P, params, n_params * sizeof(gub_params));
   gub::k_hash_expand<<<(unsigned)((n + 255) / 256), 256, 0, t->s_compute>>>(s.d_packed, (uint32_t)n, P, (uint32_t)n_params, inl ? nullptr : s.d_params, created_base, s.d_req);
+  gub::StoreArgs S;
+  if (sc && store_before(t, s.d_req, (uint32_t)n, clk, *sc, S, t->s_compute)) return -1;
   if (launch_batch(t, s.d_req, n, clk, s.d_resp, t->s_compute)) return -1;
+  if (sc && store_after(t, s.d_resp, *sc, S, t->s_compute)) return -1;
   CK(cudaEventRecord(t->compute_done[si], t->s_compute));
   CK(cudaStreamWaitEvent(t->s_d2h, t->compute_done[si], 0));
   CK(cudaMemcpyAsync(out, s.d_resp, n * sizeof(gub_resp), cudaMemcpyDeviceToHost, t->s_d2h));
   CK(cudaEventRecord(s.out_done, t->s_d2h));
   s.busy = true;
   return 0;
+}
+
+// The device address of page-locked host memory, or null when `p` is not page-locked.
+template <typename T>
+T* pinned_view(const T* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return nullptr; }
+  return a.type == cudaMemoryTypeHost ? static_cast<T*>(a.devicePointer) : nullptr;
+}
+
+}  // namespace
+
+extern "C" {
+
+int gub_submit_keys_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params, int64_t created_base,
+                          const gub_clock* clk, gub_resp* out, int* ticket) {
+  if (!t || !clk || !ticket || (n && (!packed || !out || !params))) return fail("gub_submit_keys_async: null argument");
+  if (n > 0x7FFFFFFFull || n_params > 0xFFFFFFFFull) return fail("gub_submit_keys_async: too large");
+  if (n && packed_bytes < n * sizeof(gub_kreq) + (n + 1) * 4) return fail("gub_submit_keys_async: packed buffer too small");
+  return submit_keys(t, packed, packed_bytes, n, params, n_params, created_base, clk, out, ticket, nullptr);
+}
+
+int gub_submit_keys_store_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params,
+                                int64_t created_base, const gub_clock* clk, gub_store_get_fn get, void* user, gub_resp* out,
+                                gub_store_rec* changes, uint32_t* n_changes, int* ticket) {
+  static_assert(sizeof(gub_store_rec) == 104, "gub_store_rec is 16 bytes + a gub_item");
+  if (!t || !clk || !ticket || !changes || !n_changes || (n && (!packed || !out || !params))) return fail("gub_submit_keys_store_async: null argument");
+  if (n > t->max_batch) return fail("gub_submit_keys_store_async: n = " + std::to_string(n) + " exceeds max_batch = " + std::to_string(t->max_batch) +
+                                    " (a key split over two chunks would get two records)");
+  if (n_params > 0xFFFFFFFFull) return fail("gub_submit_keys_store_async: too large");
+  if (n && packed_bytes < n * sizeof(gub_kreq) + (n + 1) * 4) return fail("gub_submit_keys_store_async: packed buffer too small");
+  if (t->fused) return fail("gub_submit_keys_store_async: not available on a table created under GUB_PATH=fused");
+  CK(cudaSetDevice(t->device));
+  StoreCall sc;
+  sc.get = get; sc.user = user; sc.changes = pinned_view(changes); sc.n_changes = pinned_view(n_changes);
+  if (!sc.changes || !sc.n_changes) return fail("gub_submit_keys_store_async: changes and n_changes must be page-locked host memory (gub_host_alloc)");
+  if (n == 0) *n_changes = 0;
+  return submit_keys(t, packed, packed_bytes, n, params, n_params, created_base, clk, out, ticket, &sc);
 }
 
 int gub_wait(gub_table* t, int ticket) {
@@ -737,13 +919,13 @@ void gub_host_free(void* p) { if (p) cudaFreeHost(p); }
 
 namespace {
 // Items parked by a batch whose probe window was full are placed before anything else reads or writes the table.
-int drain_pending(gub_table* t) {
+int drain_pending(gub_table* t, cudaStream_t st) {
   gub_clock clk;
   std::memset(&clk, 0, sizeof clk);
   clk.now_ms = INT64_MIN;  // nothing counts as expired here: only free, removed and then the earliest-expiring entries give way
   gub::FArgs A;
   fused_base_args(t, &clk, A);
-  gub::k_drain_overflow<<<1, 32>>>(A);
+  gub::k_drain_overflow<<<1, 32, 0, st>>>(A);
   CK(cudaGetLastError());
   return 0;
 }

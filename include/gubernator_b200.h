@@ -198,6 +198,45 @@ int gub_keys_layout(size_t n, size_t key_bytes, size_t* offsets_at, size_t* byte
 int gub_submit_keys_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params, size_t n_params,
                           int64_t created_base, const gub_clock* clk, gub_resp* out, int* ticket);
 
+/* ---- the Store plugin (config.go:95: Store.Get on a cache miss, Store.OnChange after an owner's update, Store.Remove when an item is
+ * deleted; algorithms.go:45-51, 78-100, 149-153, 252-254, 274-315, 382-384, 488-490) on the key-string path, one batch at a time.
+ * The device computes the batch's miss list before evaluating it and its change log after; the host calls the store.  The rule is
+ * the host layer's (gubernator_b200_host.h gub_store), at batch granularity, per distinct key:
+ *   Get       once per key that misses (absent, expired at now_ms, or past its InvalidAt), with the key's first request;
+ *             what it returns is installed before the batch is evaluated (as gub_add_items installs it);
+ *   Remove    when the item that existed at batch start was deleted: a TOKEN_BUCKET request with RESET_REMAINING anywhere among the
+ *             key's requests, or an algorithm switch by its first request (a loaded item existed when its ExpireAt >= now_ms);
+ *   OnChange  once, with the item as the batch left it, when the key is live afterwards and its last request has err_code 0 and
+ *             carries GUB_REQ_IS_OWNER. */
+enum { GUB_STORE_FOUND = 1, GUB_STORE_REMOVE = 2, GUB_STORE_CHANGE = 4 };
+typedef struct {
+  uint32_t first;   /* batch index of the key's first request (the request Store.Get receives) */
+  uint32_t last;    /* batch index of the key's last request  (the request Store.OnChange receives) */
+  uint32_t flags;   /* GUB_STORE_FOUND (Get: item filled by the callback) | GUB_STORE_REMOVE | GUB_STORE_CHANGE */
+  uint32_t _pad;
+  gub_item item;    /* key_xxh64 / key_fnv1 always set by the library; the rest per flags */
+} gub_store_rec;    /* 104 bytes */
+
+/* Store.Get for the batch's misses, called once per batch, on the calling thread (which holds the table's lock: the callback must not
+ * call into the library for this table), only when there is at least one miss.
+ * Fill misses[k].item and set GUB_STORE_FOUND for the keys the store has.  Non-zero = fail the submission: nothing is evaluated. */
+typedef int (*gub_store_get_fn)(void* user, gub_store_rec* misses, size_t n);
+
+/* gub_submit_keys_async (same batch format, same responses on the same table state, except where Store.Get returned an item) plus the
+ * Store's calls.  After gub_wait(ticket), changes[0 .. *n_changes) holds one record per key with GUB_STORE_REMOVE and/or
+ * GUB_STORE_CHANGE set, ordered by `first`; call Remove, then OnChange, for each record in turn (the host layer's order).
+ * `changes` (room for n records) and `n_changes` must be page-locked (gub_host_alloc): the device writes the records there directly,
+ * so they cross PCIe once, 104 bytes each.
+ * get == NULL (a write-behind store that never reads): fully asynchronous, like gub_submit_keys_async.
+ * get != NULL: BLOCKS until this batch's miss list is known, which is after every earlier submission on this table has finished
+ * evaluating: the pipelining of consecutive batches is lost.
+ * Refused (with text in gub_last_error()): n > max_batch (a key split over two chunks would get two records), a table created under
+ * GUB_PATH=fused, and `changes` / `n_changes` outside page-locked host memory.  Rings (gub_p2p_*) have no Store path. */
+int gub_submit_keys_store_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params,
+                                size_t n_params, int64_t created_base, const gub_clock* clk,
+                                gub_store_get_fn get, void* user,
+                                gub_resp* out, gub_store_rec* changes, uint32_t* n_changes, int* ticket);
+
 /* Page-locked host memory for request/response buffers: with these the H2D/D2H copies of gub_submit_async are truly
  * asynchronous (a Go shim allocates its batch arenas here once).  Any other host memory works too, just slower. */
 void* gub_host_alloc(size_t bytes);
