@@ -725,9 +725,9 @@ int device_view(T* host_ptr, T** dev_ptr) {
   return 0;
 }
 
-// Before the batch (host layer: gub_get_items, Store.Get, gub_add_items): the per-key dedup, the lookup of every key at its first
-// request and, with a Get callback, the miss list, the call and the installation of what the store returned.
-int store_before(gub_table* t, const gub_req* d_req, uint32_t n, const gub_clock* clk, const StoreCall& sc, gub::StoreArgs& S, cudaStream_t st) {
+// What every Store pass shares: the scratch (allocated on first use), the dedup epoch, the table and the clock.  The caller sets
+// S.reqs / S.n (and S.out before the post-pass).
+int store_args(gub_table* t, const gub_clock* clk, bool want_misses, gub::StoreArgs& S, cudaStream_t st) {
   if (store_ensure(t)) return -1;
   if (order_after_last(t, st)) return -1;  // the lookups read the table
   auto& ss = t->store;
@@ -737,54 +737,98 @@ int store_before(gub_table* t, const gub_req* d_req, uint32_t n, const gub_clock
   }
   ss.epoch++;
   std::memset(&S, 0, sizeof S);
-  S.reqs = d_req; S.n = n; S.epoch = ss.epoch; S.keys = ss.keys; S.key_mask = ss.key_entries - 1; S.kent = ss.kent; S.bstate = ss.bstate;
+  S.epoch = ss.epoch; S.keys = ss.keys; S.key_mask = ss.key_entries - 1; S.kent = ss.kent; S.bstate = ss.bstate;
   S.sel = ss.sel; S.sparse = ss.sparse; S.blk = ss.blk; S.table = t->table; S.capacity = t->capacity; S.ovf = t->ovf;
-  S.ovf_count = &t->ctl->ovf_count; S.inv = t->inv; S.now_ms = clk->now_ms; S.want_misses = sc.get ? 1u : 0u;
-  const unsigned blocks = (n + gub::STORE_THREADS - 1) / gub::STORE_THREADS;
-  gub::k_store_keys<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
-  gub::k_store_before<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
-  CK(cudaGetLastError());
-  t->last_stream = st; t->last_pending = true;
-  if (!sc.get) return 0;
+  S.ovf_count = &t->ctl->ovf_count; S.inv = t->inv; S.now_ms = clk->now_ms; S.want_misses = want_misses ? 1u : 0u;
+  return 0;
+}
+
+// The miss records k_store_before filed (a grid of `blocks`), compacted into the library's page-locked miss list.
+int store_misses(gub_table* t, unsigned blocks, uint32_t n, cudaStream_t st) {
+  auto& ss = t->store;
   gub_store_rec* d_miss;
   uint32_t* d_count;
   if (device_view(ss.h_miss, &d_miss) || device_view(ss.h_count, &d_count)) return -1;
   gub::k_store_compact<<<blocks, gub::STORE_THREADS, 0, st>>>(ss.sel, ss.sparse, ss.blk, n, d_miss, d_count);
   CK(cudaGetLastError());
   CK(cudaEventRecord(ss.misses_done, st));
-  CK(cudaEventSynchronize(ss.misses_done));
+  return 0;
+}
+
+// Store.Get on the miss list (complete: store_misses' event has been waited for), then the host's verdict for what it returned:
+// *nl loaded records (h_loaded), of which *ni items to install (h_items).
+int store_get(gub_table* t, gub_store_get_fn get, void* user, const gub_clock* clk, const char* what, uint32_t* nl_out, uint32_t* ni_out) {
+  auto& ss = t->store;
+  *nl_out = 0; *ni_out = 0;
   const uint32_t m = *(volatile uint32_t*)ss.h_count;
   if (m == 0) return 0;
-  std::vector<uint64_t> keys((size_t)m * 2);  // the callback may write the whole item; the keys are the library's
-  for (uint32_t k = 0; k < m; k++) { keys[2 * k] = ss.h_miss[k].item.key_xxh64; keys[2 * k + 1] = ss.h_miss[k].item.key_fnv1; }
-  const int rc = sc.get(sc.user, ss.h_miss, m);
-  if (rc != 0) return fail("gub_submit_keys_store_async: the store's get callback failed (" + std::to_string(rc) + "); nothing was evaluated");
+  // the callback may write the whole record; the keys and the request names (which the device indexes with) are the library's
+  std::vector<gub_store_rec> named((size_t)m);
+  std::memcpy(named.data(), ss.h_miss, (size_t)m * sizeof(gub_store_rec));
+  const int rc = get(user, ss.h_miss, m);
+  if (rc != 0) return fail(std::string(what) + ": the store's get callback failed (" + std::to_string(rc) + "); nothing was evaluated");
   uint32_t nl = 0, ni = 0;
   for (uint32_t k = 0; k < m; k++) {
     gub_store_rec& r = ss.h_miss[k];
     if (!(r.flags & GUB_STORE_FOUND)) continue;
-    r.item.key_xxh64 = keys[2 * k]; r.item.key_fnv1 = keys[2 * k + 1];
-    // the host layer's rule for a loaded item: it existed when it had not expired; the algorithm is the one the store returned
-    ss.h_loaded[nl++] = make_uint4(r.first, r.item.expire_at >= clk->now_ms ? gub::S_EXISTED : 0u, (uint32_t)r.item.algorithm, 0u);
+    r.first = named[k].first; r.last = named[k].last; r.first_shard = named[k].first_shard; r.last_shard = named[k].last_shard;
+    r.item.key_xxh64 = named[k].item.key_xxh64; r.item.key_fnv1 = named[k].item.key_fnv1;
+    // the host layer's rule for a loaded item: it existed when it had not expired; the algorithm is the one the store returned.  The
+    // record's first_shard (0 on a single table) lets a ring owner find the pass index again (k_store_loaded_ring).
+    ss.h_loaded[nl++] = make_uint4(r.first, r.item.expire_at >= clk->now_ms ? gub::S_EXISTED : 0u, (uint32_t)r.item.algorithm, (uint32_t)r.first_shard);
     if (r.item.algorithm == GUB_TOKEN_BUCKET || r.item.algorithm == GUB_LEAKY_BUCKET) ss.h_items[ni++] = to_dev(r.item);  // as gub_add_items
   }
+  *nl_out = nl; *ni_out = ni;
+  return 0;
+}
+
+// What store_get returned, installed before the pass: what gub_add_items does (place the parked inserts, then upsert the items), then the
+// verdicts.  segs: a ring owner's pass (the loaded records name their requests by source).
+int store_install(gub_table* t, uint32_t nl, uint32_t ni, const gub::StoreSegs* segs, cudaStream_t st) {
+  auto& ss = t->store;
   if (nl == 0) return 0;
   uint4* d_loaded;
   gub::DevItem* d_items;
   if (device_view(ss.h_loaded, &d_loaded) || device_view(ss.h_items, &d_items)) return -1;
-  if (ni) {  // what gub_add_items does: place the parked inserts, then upsert the items
+  if (ni) {
     if (drain_pending(t, st)) return -1;
     CK(cudaMemsetAsync(ss.d_failed, 0, 4, st));
     gub::k_add_items<<<(ni + 255) / 256, 256, 0, st>>>(t->table, t->capacity, d_items, ni, t->counters, ss.d_failed, t->inv);
   }
-  gub::k_store_loaded<<<(nl + gub::STORE_THREADS - 1) / gub::STORE_THREADS, gub::STORE_THREADS, 0, st>>>(d_loaded, nl, ss.bstate);
+  const unsigned blocks = (nl + gub::STORE_THREADS - 1) / gub::STORE_THREADS;
+  if (segs) gub::k_store_loaded_ring<<<blocks, gub::STORE_THREADS, 0, st>>>(d_loaded, nl, ss.bstate, *segs);
+  else gub::k_store_loaded<<<blocks, gub::STORE_THREADS, 0, st>>>(d_loaded, nl, ss.bstate);
   CK(cudaGetLastError());
-  if (ni) {
-    uint32_t failed = 0;
-    CK(cudaMemcpyAsync(&failed, ss.d_failed, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (failed) return fail("gub_submit_keys_store_async: table full for " + std::to_string(failed) + " items the store returned");
-  }
+  return 0;
+}
+
+// After store_install with ni > 0: fails when the table had no room for some of the items.
+int store_install_check(gub_table* t, const char* what, cudaStream_t st) {
+  uint32_t failed = 0;
+  CK(cudaMemcpyAsync(&failed, t->store.d_failed, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (failed) return fail(std::string(what) + ": table full for " + std::to_string(failed) + " items the store returned");
+  return 0;
+}
+
+// Before the batch (host layer: gub_get_items, Store.Get, gub_add_items): the per-key dedup, the lookup of every key at its first
+// request and, with a Get callback, the miss list, the call and the installation of what the store returned.
+int store_before(gub_table* t, const gub_req* d_req, uint32_t n, const gub_clock* clk, const StoreCall& sc, gub::StoreArgs& S, cudaStream_t st) {
+  if (store_args(t, clk, sc.get != nullptr, S, st)) return -1;
+  S.reqs = d_req; S.n = n;
+  const unsigned blocks = (n + gub::STORE_THREADS - 1) / gub::STORE_THREADS;
+  gub::k_store_keys<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
+  gub::k_store_before<<<blocks, gub::STORE_THREADS, 0, st>>>(S);
+  CK(cudaGetLastError());
+  t->last_stream = st; t->last_pending = true;
+  if (!sc.get) return 0;
+  if (store_misses(t, blocks, n, st)) return -1;
+  CK(cudaEventSynchronize(t->store.misses_done));
+  const char* what = "gub_submit_keys_store_async";
+  uint32_t nl, ni;
+  if (store_get(t, sc.get, sc.user, clk, what, &nl, &ni)) return -1;
+  if (store_install(t, nl, ni, nullptr, st)) return -1;
+  if (ni && store_install_check(t, what, st)) return -1;
   return 0;
 }
 
@@ -1464,6 +1508,9 @@ struct gub_p2p {
   uint32_t* h_counts = nullptr;    // pinned: {hits drained, queries drained, items made, spare} of the tick in flight
   void* nccl = nullptr;            // ncclComm_t
   uint64_t tick_bytes = 0;         // bytes all-gathered by the last tick
+  // Store steps (gub_p2p_step_keys_store_local_all), allocated by the first one: [2][world][cap] inverse map of this shard's routing by
+  // step parity (k_store_orig), read by the owners over peer access
+  uint32_t* store_orig = nullptr;
 };
 
 namespace {
@@ -1492,7 +1539,7 @@ void gub_p2p_destroy(gub_p2p* p) {
   cudaDeviceSynchronize();
   for (uint32_t r = 0; r < p->world; r++) if (p->opened[r]) cudaIpcCloseMemHandle(p->opened[r]);
   void* ptrs[] = {p->block, p->error, p->ticket, p->seg_off, p->g_reqs, p->g_resps, p->g_items, p->g_gather, p->g_count, p->g_counts_all,
-                  p->g_hist, p->g_hist_all};
+                  p->g_hist, p->g_hist_all, p->store_orig};
   for (void* q : ptrs) if (q) cudaFree(q);
   if (p->h_counts) cudaFreeHost(p->h_counts);
   if (p->h_hist) cudaFreeHost(p->h_hist);
@@ -1688,37 +1735,64 @@ int p2p_route_keys(gub_p2p* p, gub_p2p::Route* rt, const gub::P2PArgs& A, const 
   return 0;
 }
 
-// The owner side of a step.  Default: the four-kernel pipeline reading the mailbox segments in place — k_seg_wait (one warp waits
-// for the sources' flags and writes the segment offsets), the batch kernels in ring mode (responses stored straight into the
-// sources' response mailboxes), k_seg_publish (response flags).  GUB_PATH=fused: one launch of the persistent kernel instead.
+// The mailbox segments of this step as the batch kernels in ring mode read them.
+SegDesc p2p_segs(gub_p2p* p, const gub::P2PArgs& A) {
+  const uint32_t par = p->epoch & 1u;
+  SegDesc sd;
+  sd.nseg = p->world; sd.seg_off = p->seg_off;
+  for (uint32_t s = 0; s < p->world; s++) {
+    sd.reqs[s] = A.peers[p->rank].req_mb + ((size_t)par * p->world + s) * p->cap;   // what source s stored into our mailbox
+    sd.out[s] = A.peers[s].resp_mb + ((size_t)par * p->world + p->rank) * p->cap;   // NVLink stores into source s's response mailbox
+  }
+  return sd;
+}
+
+// The pieces of the owner side on the four-kernel pipeline: k_seg_wait (one warp waits for the sources' flags and writes the segment
+// offsets), the batch kernels in ring mode over as many passes as world x cap takes (responses stored straight into the sources'
+// response mailboxes), k_seg_publish (response flags).
+int p2p_seg_wait(gub_p2p* p, const gub::P2PArgs& A, cudaStream_t st) {
+  gub::k_seg_wait<<<1, 32, 0, st>>>(A, p->seg_off);
+  CK(cudaGetLastError());
+  return 0;
+}
+int p2p_eval_passes(gub_p2p* p, const gub::P2PArgs& A, const gub_clock* clk, cudaStream_t st) {
+  gub_table* t = p->t;
+  const SegDesc sd = p2p_segs(p, A);
+  const uint64_t total = (uint64_t)p->world * p->cap;
+  for (uint64_t off = 0; off < total; off += t->max_batch) {
+    const uint32_t m = (uint32_t)std::min<uint64_t>(t->max_batch, total - off);
+    if (launch_chunk(t, nullptr, m, clk, nullptr, st, p->seg_off + p->world, (uint32_t)off, &sd)) return -1;
+  }
+  return 0;
+}
+int p2p_publish_flags(gub_p2p* p, const gub::P2PArgs& A, cudaStream_t st) {
+  gub_table* t = p->t;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = (t->pdl && !t->prof) ? 1 : 0;
+  CK(cudaLaunchKernelEx(&cfg, gub::k_seg_publish, A));
+  return 0;
+}
+int p2p_publish(gub_p2p* p, const gub::P2PArgs& A, const gub_clock* clk, cudaStream_t st) {
+  if (p2p_publish_flags(p, A, st)) return -1;
+  return maybe_sweep(p->t, clk, st);
+}
+
+// The owner side of a step.  Default: the four-kernel pipeline reading the mailbox segments in place (p2p_seg_wait, p2p_eval_passes,
+// p2p_publish).  GUB_PATH=fused: one launch of the persistent kernel instead.
 int p2p_evaluate(gub_p2p* p, const gub::P2PArgs& A, const gub_clock* clk, cudaStream_t st) {
   gub_table* t = p->t;
   if (!t->fused) {
-    const uint32_t par = p->epoch & 1u;
-    SegDesc sd;
-    sd.nseg = p->world; sd.seg_off = p->seg_off;
-    for (uint32_t s = 0; s < p->world; s++) {
-      sd.reqs[s] = A.peers[p->rank].req_mb + ((size_t)par * p->world + s) * p->cap;   // what source s stored into our mailbox
-      sd.out[s] = A.peers[s].resp_mb + ((size_t)par * p->world + p->rank) * p->cap;   // NVLink stores into source s's response mailbox
-    }
-    gub::k_seg_wait<<<1, 32, 0, st>>>(A, p->seg_off);
+    if (p2p_seg_wait(p, A, st)) return -1;
     // GLOBAL requests evaluated here as owner go to the updates queue (gubernator.go:604-606, global.go:80-84).  The queue kernels
     // read the request mailboxes, so they run BEFORE the response flags go out: once a source has its answers it may route the
     // step after next into the same mailbox half.
     if (p->updates_q && gq_accumulate_segments(p, A, st)) return -1;
-    const uint64_t total = (uint64_t)p->world * p->cap;
-    for (uint64_t off = 0; off < total; off += t->max_batch) {
-      const uint32_t m = (uint32_t)std::min<uint64_t>(t->max_batch, total - off);
-      if (launch_chunk(t, nullptr, m, clk, nullptr, st, p->seg_off + p->world, (uint32_t)off, &sd)) return -1;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(1); cfg.blockDim = dim3(32); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = (t->pdl && !t->prof) ? 1 : 0;
-    CK(cudaLaunchKernelEx(&cfg, gub::k_seg_publish, A));
-    return maybe_sweep(t, clk, st);
+    if (p2p_eval_passes(p, A, clk, st)) return -1;
+    return p2p_publish(p, A, clk, st);
   }
   gub::FArgs F;
   fused_base_args(t, clk, F);
@@ -1968,6 +2042,178 @@ int gub_p2p_step_mixed_local_all(gub_p2p* const* ps, uint32_t world, const gub_r
 
 int gub_p2p_step(gub_p2p* p, const gub_req* d_reqs, size_t n, const gub_clock* clk, gub_resp* d_out, void* stream) {
   return gub_p2p_step_streams(p, d_reqs, n, clk, d_out, stream, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// A Store plugin's part in a ring step: the Get callback and every owner's change log (device views of the caller's page-locked buffers).
+struct RingStore {
+  gub_store_get_fn get = nullptr;
+  void* user = nullptr;
+  std::vector<gub_store_rec*> changes;
+  std::vector<uint32_t*> n_changes;
+};
+
+// Owner p's pass as the Store kernels read it: its mailbox segments, and every source's inverse map and routing permutation of this
+// step's parity (the sources' memory: peer access).
+gub::StoreSegs store_segs(gub_p2p* p, const gub::P2PArgs& A) {
+  const uint32_t par = p->epoch & 1u;
+  const SegDesc sd = p2p_segs(p, A);
+  gub::StoreSegs G;
+  std::memset(&G, 0, sizeof G);
+  G.nseg = p->world; G.seg_off = p->seg_off;
+  for (uint32_t s = 0; s < p->world; s++) {
+    const gub_p2p* src = p->local_peers[s];
+    G.req[s] = sd.reqs[s]; G.out[s] = sd.out[s];
+    G.orig[s] = src->store_orig + ((size_t)par * p->world + p->rank) * p->cap;
+    G.perm[s] = src->rt[par].perm;
+  }
+  return G;
+}
+
+// p2p_local_all with the Store's pre- and post-pass on every owner (arguments checked by the caller):
+//   1. every routing, each followed by its inverse map (k_store_orig);   2. local_phase_sync;
+//   3. per owner: k_seg_wait, the pre-pass and, with a Get, the miss list compacted into the table's page-locked buffer;
+//   4. with a Get: wait for every miss list, call Get per owner in rank order, then install what it returned on every owner;
+//   5. per owner: the ring-mode passes, the post-pass straight into changes[r], k_seg_publish.  The post-pass reads the request
+//      mailbox, so it runs before the response flags go out (a source that has its answers may route step e + 2 into that half);
+//   6. local_phase_sync;   7. every collect.
+// A failing Get (or a table that cannot take the items the store returned) fails the call, but every owner still publishes its flags
+// (without evaluating) and every source collects, so that the ring stays in step.
+int p2p_local_all_store(gub_p2p* const* ps, uint32_t world, const Ingest* in, const size_t* n, const gub_clock* clk, const RingStore& rs,
+                        gub_resp* const* d_out, void* const* streams) {
+  const char* what = "gub_p2p_step_keys_store_local_all";
+  const uint32_t pass = world * ps[0]->cap;  // launch size of the Store kernels; the pass itself is seg_off[world] <= pass
+  const unsigned blocks = (pass + gub::STORE_THREADS - 1) / gub::STORE_THREADS;
+  for (uint32_t r = 0; r < world; r++) {
+    gub_p2p* p = ps[r];
+    const cudaStream_t st = (cudaStream_t)streams[r];
+    if (p2p_phase_route(p, in[r], n[r], st, st)) return -1;
+    std::lock_guard<std::mutex> lk(p->t->mu);
+    CK(cudaSetDevice(p->t->device));
+    if (n[r]) {
+      gub::k_store_orig<<<(unsigned)((n[r] + 255) / 256), 256, 0, st>>>(p->rt[p->epoch & 1u].perm, (uint32_t)n[r], p->cap,
+                                                                         p->store_orig + (size_t)(p->epoch & 1u) * world * p->cap);
+      CK(cudaGetLastError());
+    }
+  }
+  if (local_phase_sync(ps, world, streams)) return -1;
+  std::vector<gub::StoreArgs> S(world);
+  std::vector<gub::StoreSegs> G(world);
+  for (uint32_t r = 0; r < world; r++) {
+    gub_p2p* p = ps[r];
+    gub_table* t = p->t;
+    const cudaStream_t st = (cudaStream_t)streams[r];
+    std::lock_guard<std::mutex> lk(t->mu);
+    CK(cudaSetDevice(t->device));
+    gub::P2PArgs A;
+    p2p_args(p, A);
+    if (order_after_last(t, st)) return -1;
+    if (p2p_seg_wait(p, A, st)) return -1;
+    if (store_args(t, clk, rs.get != nullptr, S[r], st)) return -1;
+    S[r].n = pass;
+    G[r] = store_segs(p, A);
+    gub::k_store_keys_ring<<<blocks, gub::STORE_THREADS, 0, st>>>(S[r], G[r]);
+    gub::k_store_before_ring<<<blocks, gub::STORE_THREADS, 0, st>>>(S[r], G[r]);
+    CK(cudaGetLastError());
+    t->last_stream = st; t->last_pending = true;
+    if (rs.get && store_misses(t, blocks, pass, st)) return -1;
+  }
+  bool failed = false;
+  if (rs.get) {
+    std::vector<uint32_t> nl(world, 0), ni(world, 0);
+    for (uint32_t r = 0; r < world; r++) {
+      CK(cudaSetDevice(ps[r]->t->device));
+      CK(cudaEventSynchronize(ps[r]->t->store.misses_done));
+    }
+    for (uint32_t r = 0; r < world && !failed; r++) {
+      std::lock_guard<std::mutex> lk(ps[r]->t->mu);
+      failed = store_get(ps[r]->t, rs.get, rs.user, clk, what, &nl[r], &ni[r]) != 0;
+    }
+    for (uint32_t r = 0; r < world && !failed; r++) {
+      std::lock_guard<std::mutex> lk(ps[r]->t->mu);
+      CK(cudaSetDevice(ps[r]->t->device));
+      failed = store_install(ps[r]->t, nl[r], ni[r], &G[r], (cudaStream_t)streams[r]) != 0;
+    }
+    for (uint32_t r = 0; r < world && !failed; r++) {
+      if (!ni[r]) continue;
+      std::lock_guard<std::mutex> lk(ps[r]->t->mu);
+      CK(cudaSetDevice(ps[r]->t->device));
+      failed = store_install_check(ps[r]->t, what, (cudaStream_t)streams[r]) != 0;
+    }
+  }
+  const std::string err = failed ? g_err : std::string();
+  for (uint32_t r = 0; r < world; r++) {
+    gub_p2p* p = ps[r];
+    gub_table* t = p->t;
+    const cudaStream_t st = (cudaStream_t)streams[r];
+    std::lock_guard<std::mutex> lk(t->mu);
+    CK(cudaSetDevice(t->device));
+    gub::P2PArgs A;
+    p2p_args(p, A);
+    if (failed) {
+      if (p2p_publish_flags(p, A, st)) return -1;
+      continue;
+    }
+    if (p2p_eval_passes(p, A, clk, st)) return -1;
+    gub::k_store_after_ring<<<blocks, gub::STORE_THREADS, 0, st>>>(S[r], G[r]);
+    gub::k_store_compact<<<blocks, gub::STORE_THREADS, 0, st>>>(t->store.sel, t->store.sparse, t->store.blk, pass, rs.changes[r], rs.n_changes[r]);
+    CK(cudaGetLastError());
+    if (p2p_publish(p, A, clk, st)) return -1;
+    t->last_stream = st; t->last_pending = true;
+  }
+  if (local_phase_sync(ps, world, streams)) return -1;
+  for (uint32_t r = 0; r < world; r++) if (p2p_phase_collect(ps[r], n[r], d_out[r], (cudaStream_t)streams[r], (cudaStream_t)streams[r])) return -1;
+  if (failed) return fail(err);
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int gub_p2p_step_keys_store_local_all(gub_p2p* const* ps, uint32_t world, const void* const* d_packed, const size_t* packed_bytes,
+                                      const size_t* n, const gub_params* params, size_t n_params, int64_t created_base,
+                                      const gub_clock* clk, gub_store_get_fn get, void* user, gub_resp* const* d_out,
+                                      gub_store_rec* const* changes, uint32_t* const* n_changes, void* const* streams) {
+  const std::string what = "gub_p2p_step_keys_store_local_all";
+  if (!ps || !d_packed || !packed_bytes || !n || !d_out || !changes || !n_changes || !streams || world == 0) return fail(what + ": bad argument");
+  std::vector<Ingest> in(world);
+  RingStore rs;
+  rs.get = get; rs.user = user;
+  for (uint32_t r = 0; r < world; r++) {
+    gub_p2p* p = ps[r];
+    if (p2p_step_keys_check(p, d_packed[r], packed_bytes[r], n[r], params, n_params, clk, d_out[r], what.c_str())) return -1;
+    if (p->world != world || p->rank != r) return fail(what + ": ps[" + std::to_string(r) + "] is not rank " + std::to_string(r) + " of a ring of " + std::to_string(world));
+    if (p->t->fused) return fail(what + ": not available on tables created under GUB_PATH=fused");
+    if (p->hits_q || p->updates_q) return fail(what + ": not available on a ring with GLOBAL enabled (the owner-side application of a tick's hits has no change log)");
+    bool local = p->group != nullptr;
+    for (uint32_t s = 0; s < world; s++) local = local && p->local_peers[s] == ps[s];
+    if (!local) return fail(what + ": the shards must be connected with gub_p2p_connect_local");
+    if ((uint64_t)world * p->cap > p->t->max_batch)
+      return fail(what + ": world x cap = " + std::to_string((uint64_t)world * p->cap) + " exceeds an owner's pass of " + std::to_string(p->t->max_batch) +
+                  " requests (a key split over two passes would get two records)");
+    CK(cudaSetDevice(p->t->device));
+    if (!changes[r] || !n_changes[r]) return fail(what + ": null argument");
+    rs.changes.push_back(pinned_view(changes[r]));
+    rs.n_changes.push_back(pinned_view(n_changes[r]));
+    if (!rs.changes.back() || !rs.n_changes.back()) return fail(what + ": changes and n_changes must be page-locked host memory (gub_host_alloc)");
+    in[r] = keys_ingest(d_packed[r], packed_bytes[r], params, n_params, created_base);
+  }
+  for (uint32_t r = 0; r < world; r++) {  // the first Store step allocates (and synchronises the device) before anything is enqueued
+    gub_p2p* p = ps[r];
+    std::lock_guard<std::mutex> lk(p->t->mu);
+    CK(cudaSetDevice(p->t->device));
+    if (store_ensure(p->t)) return -1;
+    if (!p->store_orig) {
+      const size_t bytes = (size_t)2 * world * p->cap * 4;
+      CK(cudaMalloc(&p->store_orig, bytes));
+      CK(cudaMemset(p->store_orig, 0, bytes));
+    }
+  }
+  return p2p_local_all_store(ps, world, in.data(), n, clk, rs, d_out, streams);
 }
 
 }  // extern "C"

@@ -18,6 +18,8 @@
 //                    output may be host memory (the caller's page-locked buffers).
 // A record at index i is filed only by thread i (the key's work runs at its first request, not its last, for that reason), so each block
 // counts what it filed and the compaction finds a block's output offset by summing the counts of the blocks before it.
+// On a ring (gub_p2p_step_keys_store_local_all) the same passes run per owner over its mailbox segments (StoreRing: the *_ring kernels),
+// and k_store_orig gives every source an inverse map of its routing so that an owner can name each request by (source, source index).
 #pragma once
 #include "gub_kernels.cuh"
 
@@ -91,7 +93,7 @@ __device__ __forceinline__ void store_item(const Bucket& b, int64_t inv_at, gub_
 }
 
 __device__ __forceinline__ void store_rec_init(gub_store_rec& r, uint32_t first, uint32_t last, uint32_t flags, const gub_req& rq) {
-  r.first = first; r.last = last; r.flags = flags; r._pad = 0;
+  r.first = first; r.last = last; r.flags = flags; r.first_shard = 0; r.last_shard = 0;
   r.item.key_xxh64 = rq.key_xxh64; r.item.key_fnv1 = rq.key_fnv1;
   r.item.algorithm = 0; r.item.status = 0; r.item.limit = 0; r.item.duration = 0; r.item.remaining = 0; r.item.remaining_f = 0.0;
   r.item.stamp = 0; r.item.burst = 0; r.item.expire_at = 0; r.item.invalid_at = 0;
@@ -108,10 +110,77 @@ __device__ __forceinline__ void store_block_count(bool filed, uint32_t* blk) {
   if (threadIdx.x == 0) blk[blockIdx.x] = s_cnt;
 }
 
-__global__ void __launch_bounds__(STORE_THREADS) k_store_keys(const StoreArgs S) {
+// ---- where the requests of a pass live ---------------------------------------------------------------------------------------
+// The kernels below are written once over an input.  StoreDense: a single table's batch (StoreArgs::reqs / out; a record names its
+// requests by batch index).  StoreRing: an owner's pass over its mailbox segments (gub_p2p_step_keys_store_local_all): pass request
+// g is record g - off[s] of source s's segment, its response sits in source s's response mailbox, and a record names a request by
+// (source shard, index in that source's ingest batch), read from the source's inverse map.  StoreArgs::n is then the launch size
+// (world x cap) and the pass size is seg_off[world], written by k_seg_wait.
+struct StoreDense {
+  const StoreArgs& S;
+  __device__ __forceinline__ uint32_t n() const { return S.n; }
+  __device__ __forceinline__ bool live(uint32_t) const { return true; }
+  __device__ __forceinline__ gub_req req(uint32_t i) const { return S.reqs[i]; }
+  __device__ __forceinline__ const gub_req* at(uint32_t i) const { return S.reqs + i; }
+  __device__ __forceinline__ uint64_t ld(const uint64_t* p) const { return *p; }
+  __device__ __forceinline__ uint32_t behavior(uint32_t i) const { return S.reqs[i].behavior; }
+  __device__ __forceinline__ uint32_t err_code(uint32_t i) const { return S.out[i].err_code; }
+  __device__ __forceinline__ void name(gub_store_rec&) const {}
+};
+
+// The segments of an owner's pass (device pointers of this step's parity; `orig` and `perm` are the sources' memory, read over peer access).
+struct StoreSegs {
+  uint32_t nseg;
+  const uint32_t* seg_off;            // [nseg + 1] prefix sums of the segments (k_seg_wait)
+  const gub_req* req[MAX_SHARDS];     // source s's segment of our request mailbox
+  const gub_resp* out[MAX_SHARDS];    // our part of source s's response mailbox
+  const uint32_t* orig[MAX_SHARDS];   // source s's inverse map, our row: orig[s][pos] = index in s's ingest batch (k_store_orig)
+  const uint32_t* perm[MAX_SHARDS];   // source s's routing permutation: perm[s][i] = owner << 24 | pos (k_store_loaded_ring)
+};
+// The segment table in shared memory: a dynamic index into the kernel parameters would copy them to local memory.
+struct StoreSegShared { const gub_req* req[MAX_SHARDS]; const gub_resp* out[MAX_SHARDS]; const uint32_t* orig[MAX_SHARDS]; const uint32_t* perm[MAX_SHARDS]; uint32_t off[MAX_SHARDS + 1]; uint32_t nseg; };
+
+// Block-wide (a barrier): fills the shared segment table.
+__device__ __forceinline__ const StoreSegShared* store_segs_open(const StoreSegs& G) {
+  __shared__ StoreSegShared s_seg;
+#pragma unroll
+  for (int k = 0; k < MAX_SHARDS; k++) {
+    if (threadIdx.x == (uint32_t)k && (uint32_t)k < G.nseg) { s_seg.req[k] = G.req[k]; s_seg.out[k] = G.out[k]; s_seg.orig[k] = G.orig[k]; s_seg.perm[k] = G.perm[k]; }
+  }
+  if (threadIdx.x <= G.nseg) s_seg.off[threadIdx.x] = __ldcg(G.seg_off + threadIdx.x);
+  if (threadIdx.x == 0) s_seg.nseg = G.nseg;
+  __syncthreads();
+  return &s_seg;
+}
+
+struct StoreRing {
+  const StoreArgs& S;
+  const StoreSegShared* T;
+  __device__ __forceinline__ uint32_t seg_of(uint32_t g) const { uint32_t s = 0; while (s + 1 < T->nseg && g >= T->off[s + 1]) s++; return s; }
+  __device__ __forceinline__ const gub_req* at(uint32_t g) const { const uint32_t s = seg_of(g); return T->req[s] + (g - T->off[s]); }
+  __device__ __forceinline__ uint32_t n() const { return min(T->off[T->nseg], S.n); }
+  __device__ __forceinline__ bool live(uint32_t i) const { return i < n(); }
+  // records other GPUs stored into this GPU's memory: L2 is the point of coherence
+  __device__ __forceinline__ gub_req req(uint32_t i) const { return load_req_cg(at(i)); }
+  __device__ __forceinline__ uint64_t ld(const uint64_t* p) const { return __ldcg(p); }
+  __device__ __forceinline__ uint32_t behavior(uint32_t i) const { return __ldcg(&at(i)->behavior); }
+  __device__ __forceinline__ uint32_t err_code(uint32_t i) const {
+    const uint32_t s = seg_of(i);
+    return __ldcg(&T->out[s][i - T->off[s]].err_code);
+  }
+  // pass indices -> (source shard, index in the source's ingest batch)
+  __device__ __forceinline__ void name(gub_store_rec& r) const {
+    const uint32_t sf = seg_of(r.first), sl = seg_of(r.last);
+    r.first_shard = (uint16_t)sf; r.first = __ldcg(T->orig[sf] + (r.first - T->off[sf]));
+    r.last_shard = (uint16_t)sl; r.last = __ldcg(T->orig[sl] + (r.last - T->off[sl]));
+  }
+};
+
+template <typename In>
+__device__ __forceinline__ void store_keys(const StoreArgs& S, const In& in) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= S.n) return;
-  const gub_req rq = S.reqs[i];
+  if (i >= in.n()) return;
+  const gub_req rq = in.req(i);
   const uint64_t key = remap_key(rq.key_xxh64), tag = rq.key_fnv1 >> 8;
   const unsigned long long ep = (unsigned long long)S.epoch << 32;
   uint32_t pos = (uint32_t)(key ^ (key >> 31)) & S.key_mask;
@@ -124,8 +193,8 @@ __global__ void __launch_bounds__(STORE_THREADS) k_store_keys(const StoreArgs S)
       c = old;
     }
     if ((c >> 32) == (unsigned long long)S.epoch) {
-      const gub_req& o = S.reqs[(uint32_t)c];
-      if (remap_key(o.key_xxh64) == key && (o.key_fnv1 >> 8) == tag) break;
+      const gub_req* o = in.at((uint32_t)c);
+      if (remap_key(in.ld(&o->key_xxh64)) == key && (in.ld(&o->key_fnv1) >> 8) == tag) break;
     }
     pos = (pos + 1) & S.key_mask;
   }
@@ -135,28 +204,75 @@ __global__ void __launch_bounds__(STORE_THREADS) k_store_keys(const StoreArgs S)
   if (rq.algorithm == GUB_TOKEN_BUCKET && (rq.behavior & GUB_BEHAVIOR_RESET_REMAINING)) atomicMax(&S.keys[pos].reset, ep | 1u);
 }
 
-__global__ void __launch_bounds__(STORE_THREADS) k_store_before(const StoreArgs S) {
+template <typename In>
+__device__ __forceinline__ void store_before(const StoreArgs& S, const In& in) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   bool filed = false;
   if (i < S.n) {
-    const StoreKey k = S.keys[S.kent[i]];
-    if (skey_first(k) == i) {
-      const gub_req rq = S.reqs[i];
-      Bucket b;
-      int64_t inv_at;
-      const bool found = store_lookup(S, remap_key(rq.key_xxh64), rq.key_fnv1 >> 8, b, inv_at);
-      S.bstate[i] = StoreState{found ? S_EXISTED : 0u, (b.flags & F_LEAKY) ? (uint32_t)GUB_LEAKY_BUCKET : (uint32_t)GUB_TOKEN_BUCKET};
-      if (!found && S.want_misses) {
-        gub_store_rec r;
-        store_rec_init(r, i, (uint32_t)k.last, 0u, rq);
-        S.sparse[i] = r;
-        filed = true;
+    if (in.live(i)) {
+      const StoreKey k = S.keys[S.kent[i]];
+      if (skey_first(k) == i) {
+        const gub_req rq = in.req(i);
+        Bucket b;
+        int64_t inv_at;
+        const bool found = store_lookup(S, remap_key(rq.key_xxh64), rq.key_fnv1 >> 8, b, inv_at);
+        S.bstate[i] = StoreState{found ? S_EXISTED : 0u, (b.flags & F_LEAKY) ? (uint32_t)GUB_LEAKY_BUCKET : (uint32_t)GUB_TOKEN_BUCKET};
+        if (!found && S.want_misses) {
+          gub_store_rec r;
+          store_rec_init(r, i, (uint32_t)k.last, 0u, rq);
+          in.name(r);
+          S.sparse[i] = r;
+          filed = true;
+        }
       }
     }
     S.sel[i] = filed ? 1 : 0;
   }
   store_block_count(filed, S.blk);
 }
+
+template <typename In>
+__device__ __forceinline__ void store_after(const StoreArgs& S, const In& in) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  bool filed = false;
+  if (i < S.n) {
+    if (in.live(i)) {
+      const StoreKey k = S.keys[S.kent[i]];
+      if (skey_first(k) == i) {
+        const gub_req rq = in.req(i);
+        const uint32_t last = (uint32_t)k.last;
+        Bucket b;
+        int64_t inv_at;
+        const bool live = store_lookup(S, remap_key(rq.key_xxh64), rq.key_fnv1 >> 8, b, inv_at);
+        const StoreState bs = S.bstate[i];
+        // Store.Remove (algorithms.go:78-83, 91-100, 308-315): the item that existed was deleted
+        const bool switched = (int32_t)bs.algorithm != (int32_t)rq.algorithm && rq.algorithm <= 1u;
+        const bool reset = k.reset == (((unsigned long long)S.epoch << 32) | 1ull);
+        // Store.OnChange (algorithms.go:149, 252): owner requests only
+        const bool change = live && in.err_code(last) == 0 && (in.behavior(last) & GUB_REQ_IS_OWNER);
+        const uint32_t flags = ((bs.existed & S_EXISTED) && (switched || reset) ? (uint32_t)GUB_STORE_REMOVE : 0u) | (change ? (uint32_t)GUB_STORE_CHANGE : 0u);
+        if (flags) {
+          gub_store_rec r;
+          store_rec_init(r, i, last, flags, rq);
+          if (change) {
+            store_item(b, inv_at, r.item);
+            r.item.key_xxh64 = rq.key_xxh64; r.item.key_fnv1 = rq.key_fnv1;
+          }
+          in.name(r);
+          S.sparse[i] = r;
+          filed = true;
+        }
+      }
+    }
+    S.sel[i] = filed ? 1 : 0;
+  }
+  store_block_count(filed, S.blk);
+}
+
+// Single table (gub_submit_keys_store_async).
+__global__ void __launch_bounds__(STORE_THREADS) k_store_keys(const StoreArgs S) { store_keys(S, StoreDense{S}); }
+__global__ void __launch_bounds__(STORE_THREADS) k_store_before(const StoreArgs S) { store_before(S, StoreDense{S}); }
+__global__ void __launch_bounds__(STORE_THREADS) k_store_after(const StoreArgs S) { store_after(S, StoreDense{S}); }
 
 // loaded[k] = (first, existed, algorithm, -) for the items Store.Get returned
 __global__ void __launch_bounds__(STORE_THREADS) k_store_loaded(const uint4* loaded, uint32_t m, StoreState* bstate) {
@@ -166,39 +282,34 @@ __global__ void __launch_bounds__(STORE_THREADS) k_store_loaded(const uint4* loa
   bstate[l.x] = StoreState{l.y, l.z};
 }
 
-__global__ void __launch_bounds__(STORE_THREADS) k_store_after(const StoreArgs S) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  bool filed = false;
-  if (i < S.n) {
-    const StoreKey k = S.keys[S.kent[i]];
-    if (skey_first(k) == i) {
-      const gub_req rq = S.reqs[i];
-      const uint32_t last = (uint32_t)k.last;
-      Bucket b;
-      int64_t inv_at;
-      const bool live = store_lookup(S, remap_key(rq.key_xxh64), rq.key_fnv1 >> 8, b, inv_at);
-      const StoreState bs = S.bstate[i];
-      // Store.Remove (algorithms.go:78-83, 91-100, 308-315): the item that existed was deleted
-      const bool switched = (int32_t)bs.algorithm != (int32_t)rq.algorithm && rq.algorithm <= 1u;
-      const bool reset = k.reset == (((unsigned long long)S.epoch << 32) | 1ull);
-      // Store.OnChange (algorithms.go:149, 252): owner requests only
-      const bool change = live && S.out[last].err_code == 0 && (S.reqs[last].behavior & GUB_REQ_IS_OWNER);
-      const uint32_t flags = ((bs.existed & S_EXISTED) && (switched || reset) ? (uint32_t)GUB_STORE_REMOVE : 0u) | (change ? (uint32_t)GUB_STORE_CHANGE : 0u);
-      if (flags) {
-        gub_store_rec r;
-        store_rec_init(r, i, last, flags, rq);
-        if (change) {
-          store_item(b, inv_at, r.item);
-          r.item.key_xxh64 = rq.key_xxh64; r.item.key_fnv1 = rq.key_fnv1;
-        }
-        S.sparse[i] = r;
-        filed = true;
-      }
-    }
-    S.sel[i] = filed ? 1 : 0;
-  }
-  store_block_count(filed, S.blk);
+// An owner's pass over its mailbox segments (gub_p2p_step_keys_store_local_all); S.n = world x cap, the grid's size.
+__global__ void __launch_bounds__(STORE_THREADS) k_store_keys_ring(const StoreArgs S, const StoreSegs G) { store_keys(S, StoreRing{S, store_segs_open(G)}); }
+__global__ void __launch_bounds__(STORE_THREADS) k_store_before_ring(const StoreArgs S, const StoreSegs G) { store_before(S, StoreRing{S, store_segs_open(G)}); }
+__global__ void __launch_bounds__(STORE_THREADS) k_store_after_ring(const StoreArgs S, const StoreSegs G) { store_after(S, StoreRing{S, store_segs_open(G)}); }
+
+// loaded[k] = (first, existed, algorithm, first_shard) for the items Store.Get returned: the record names the key's first request by
+// source, so the pass index is found through that source's routing permutation (pass index = seg_off[s] + its mailbox position).
+__global__ void __launch_bounds__(STORE_THREADS) k_store_loaded_ring(const uint4* loaded, uint32_t m, StoreState* bstate, const StoreSegs G) {
+  const StoreSegShared* T = store_segs_open(G);
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= m) return;
+  const uint4 l = loaded[k];
+  const uint32_t g = T->off[l.w] + (__ldcg(T->perm[l.w] + l.x) & 0xFFFFFFu);
+  bstate[g] = StoreState{l.y, l.z};
 }
+
+// Source side of a ring Store step, after its routing: orig[o * cap + pos] = i for every perm[i] = o << 24 | pos, so that owner o can
+// name the request it finds at position pos of our segment.
+__global__ void __launch_bounds__(256) k_store_orig(const uint32_t* perm, uint32_t n, uint32_t cap, uint32_t* orig) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t pk = __ldg(perm + i);
+  orig[(size_t)(pk >> 24) * cap + (pk & 0xFFFFFFu)] = i;
+}
+
+// gub_store_rec's layout in 32-bit words and above.
+struct StoreRecWords { uint32_t first, last, flags, shards; gub_item item; };
+static_assert(sizeof(StoreRecWords) == sizeof(gub_store_rec), "gub_store_rec layout");
 
 // out[0 .. *out_count) = the filed records in index order.  Same grid as the pass that filed them.
 __global__ void __launch_bounds__(STORE_THREADS) k_store_compact(const uint8_t* sel, const gub_store_rec* sparse, const uint32_t* blk, uint32_t n,
@@ -219,7 +330,10 @@ __global__ void __launch_bounds__(STORE_THREADS) k_store_compact(const uint8_t* 
     if (w < warp) before += s_wcnt[w];
     total += s_wcnt[w];
   }
-  if (p) out[base + before + (uint32_t)__popc(bal & ((1u << lane) - 1u))] = sparse[i];
+  if (p) {  // copied as whole 32-bit words (first_shard / last_shard are the two halves of one): 16-bit moves would cost more instructions
+    const StoreRecWords* src = reinterpret_cast<const StoreRecWords*>(sparse) + i;
+    reinterpret_cast<StoreRecWords*>(out)[base + before + (uint32_t)__popc(bal & ((1u << lane) - 1u))] = *src;
+  }
   if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *out_count = base + total;
 }
 

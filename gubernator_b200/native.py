@@ -28,10 +28,22 @@ PARAMS_DTYPE = np.dtype([("limit", "<i8"), ("duration", "<i8"), ("burst", "<i8")
 assert CREQ_DTYPE.itemsize == 32 and PARAMS_DTYPE.itemsize == 32
 assert REQ_DTYPE.itemsize == 64 and RESP_DTYPE.itemsize == 32 and CLOCK_DTYPE.itemsize == 104 and ITEM_DTYPE.itemsize == 88
 STORE_FOUND, STORE_REMOVE, STORE_CHANGE = 1, 2, 4
-STORE_REC_DTYPE = np.dtype([("first", "<u4"), ("last", "<u4"), ("flags", "<u4"), ("_pad", "<u4"), ("item", ITEM_DTYPE)])  # gub_store_rec
+STORE_REC_DTYPE = np.dtype([("first", "<u4"), ("last", "<u4"), ("flags", "<u4"), ("first_shard", "<u2"), ("last_shard", "<u2"),
+                            ("item", ITEM_DTYPE)])  # gub_store_rec
 assert STORE_REC_DTYPE.itemsize == 104
 # gub_store_get_fn: (user, misses, n) -> 0 = ok
 STORE_GET_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
+
+
+def _store_get_fn(get):
+    """A STORE_GET_FN over get(misses) -> None | int (misses: a STORE_REC_DTYPE view of the library's miss list, valid during the call)."""
+    if get is None:
+        return STORE_GET_FN()
+
+    def _get(_user, misses_ptr, m):
+        return int(get(np.frombuffer((C.c_char * (m * STORE_REC_DTYPE.itemsize)).from_address(misses_ptr), dtype=STORE_REC_DTYPE)) or 0)
+    return STORE_GET_FN(_get)
+
 
 EXPORTS = ["gub_create", "gub_destroy", "gub_last_error", "gub_abi_version", "gub_submit", "gub_submit_device", "gub_submit_device_n", "gub_submit_compact", "gub_submit_compact_async",
            "gub_pipeline_depth", "gub_submit_async", "gub_wait", "gub_host_alloc", "gub_host_free", "gub_clock_fill",
@@ -43,7 +55,7 @@ EXPORTS = ["gub_create", "gub_destroy", "gub_last_error", "gub_abi_version", "gu
            "gub_p2p_connect_local", "gub_p2p_step", "gub_p2p_step_streams", "gub_p2p_status", "gub_p2p_enable_global", "gub_nccl_unique_id",
            "gub_p2p_nccl_init", "gub_p2p_nccl_init_local", "gub_global_tick", "gub_gq_dropped", "gub_set_sweep", "gub_set_trace", "gub_get_trace", "gub_get_trace_raw", "gub_get_ktrace", "gub_keys_layout", "gub_submit_keys_async", "gub_global_tick_local_all", "gub_p2p_step_local_all",
            "gub_p2p_step_keys", "gub_p2p_step_keys_local_all", "gub_p2p_step_mixed_local_all",
-           "gub_submit_keys_store_async"]
+           "gub_submit_keys_store_async", "gub_p2p_step_keys_store_local_all"]
 
 
 class Config(C.Structure):
@@ -144,6 +156,7 @@ _LATE_ARGTYPES = {
     "gub_p2p_step_keys_local_all": [_pvp, C.c_uint32, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, _pvp, _pvp],
     "gub_p2p_step_mixed_local_all": [_pvp, C.c_uint32, _pvp, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, _pvp, _pvp],
     "gub_submit_keys_store_async": [_vp, _vp, _sz, _sz, _vp, _sz, C.c_int64, _vp, STORE_GET_FN, _vp, _vp, _vp, _vp, C.POINTER(C.c_int)],
+    "gub_p2p_step_keys_store_local_all": [_pvp, C.c_uint32, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, STORE_GET_FN, _vp, _pvp, _pvp, _pvp, _pvp],
 }
 
 
@@ -342,15 +355,10 @@ class Table:
         a STORE_REC_DTYPE view of the library's miss list, valid during the call only); a non-zero return fails the submission.
         changes_ptr (room for n STORE_REC_DTYPE records) and n_changes_ptr (uint32) must be page-locked (PinnedArray); after wait(),
         they hold one record per key with STORE_REMOVE and/or STORE_CHANGE, ordered by `first`.  Returns a ticket for wait()."""
-        cb = None
-        if get is not None:
-            def _get(_user, misses_ptr, m):
-                rc = get(np.frombuffer((C.c_char * (m * STORE_REC_DTYPE.itemsize)).from_address(misses_ptr), dtype=STORE_REC_DTYPE))
-                return int(rc or 0)
-            cb = STORE_GET_FN(_get)
+        cb = _store_get_fn(get)
         tk = C.c_int(-1)
         _check(_entry("gub_submit_keys_store_async")(self._h, packed_ptr, packed_bytes, n, params_ptr, n_params, int(created_base), clk.ctypes.data,
-                                                     cb if cb is not None else STORE_GET_FN(), None, out_ptr, changes_ptr, n_changes_ptr, C.byref(tk)),
+                                                     cb, None, out_ptr, changes_ptr, n_changes_ptr, C.byref(tk)),
                "gub_submit_keys_store_async")
         return tk.value
 
@@ -530,6 +538,22 @@ def p2p_step_mixed_local_all(p2ps, req_ptrs, packed_ptrs, packed_bytes, ns, para
                                               (C.c_size_t * W)(*packed_bytes), (C.c_size_t * W)(*ns), params.ctypes.data if len(params) else None,
                                               len(params), int(created_base), clk.ctypes.data, (C.c_void_p * W)(*out_ptrs), (C.c_void_p * W)(*streams)),
            "gub_p2p_step_mixed_local_all")
+
+
+def p2p_step_keys_store_local_all(p2ps, packed_ptrs, packed_bytes, ns, params, created_base, clk, get, out_ptrs, changes_ptrs, n_changes_ptrs,
+                                  streams):
+    """p2p_step_keys_local_all with a Store plugin (gub_p2p_step_keys_store_local_all).  get: None (a store that never reads) or a
+    callable get(misses) -> None | int, called once per owner that has misses, in rank order, as for Table.submit_keys_store_async; a
+    miss names its request by (first_shard, first).  changes_ptrs[r] (room for world x cap STORE_REC_DTYPE records) and
+    n_changes_ptrs[r] (uint32) must be page-locked (PinnedArray): owner r's change log, valid once streams[r] has completed the step."""
+    W = len(p2ps)
+    params = _params_array(params)
+    cb = _store_get_fn(get)
+    _check(_entry("gub_p2p_step_keys_store_local_all")((C.c_void_p * W)(*[p._h for p in p2ps]), W, (C.c_void_p * W)(*packed_ptrs),
+                                                   (C.c_size_t * W)(*packed_bytes), (C.c_size_t * W)(*ns), params.ctypes.data if len(params) else None,
+                                                   len(params), int(created_base), clk.ctypes.data, cb, None, (C.c_void_p * W)(*out_ptrs),
+                                                   (C.c_void_p * W)(*changes_ptrs), (C.c_void_p * W)(*n_changes_ptrs), (C.c_void_p * W)(*streams)),
+           "gub_p2p_step_keys_store_local_all")
 
 
 def global_tick_local_all(p2ps, clk, now_ms, streams):

@@ -213,7 +213,7 @@ typedef struct {
   uint32_t first;   /* batch index of the key's first request (the request Store.Get receives) */
   uint32_t last;    /* batch index of the key's last request  (the request Store.OnChange receives) */
   uint32_t flags;   /* GUB_STORE_FOUND (Get: item filled by the callback) | GUB_STORE_REMOVE | GUB_STORE_CHANGE */
-  uint32_t _pad;
+  uint16_t first_shard, last_shard;  /* rings: the shard whose ingest batch `first` / `last` index; 0 on a single table */
   gub_item item;    /* key_xxh64 / key_fnv1 always set by the library; the rest per flags */
 } gub_store_rec;    /* 104 bytes */
 
@@ -231,7 +231,8 @@ typedef int (*gub_store_get_fn)(void* user, gub_store_rec* misses, size_t n);
  * get != NULL: BLOCKS until this batch's miss list is known, which is after every earlier submission on this table has finished
  * evaluating: the pipelining of consecutive batches is lost.
  * Refused (with text in gub_last_error()): n > max_batch (a key split over two chunks would get two records), a table created under
- * GUB_PATH=fused, and `changes` / `n_changes` outside page-locked host memory.  Rings (gub_p2p_*) have no Store path. */
+ * GUB_PATH=fused, and `changes` / `n_changes` outside page-locked host memory.  Rings driven from one process: see
+ * gub_p2p_step_keys_store_local_all. */
 int gub_submit_keys_store_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n, const gub_params* params,
                                 size_t n_params, int64_t created_base, const gub_clock* clk,
                                 gub_store_get_fn get, void* user,
@@ -407,6 +408,34 @@ int gub_p2p_step_keys_local_all(gub_p2p* const* ps, uint32_t world, const void* 
 int gub_p2p_step_mixed_local_all(gub_p2p* const* ps, uint32_t world, const gub_req* const* d_reqs, const void* const* d_packed,
                                  const size_t* packed_bytes, const size_t* n, const gub_params* params, size_t n_params,
                                  int64_t created_base, const gub_clock* clk, gub_resp* const* d_out, void* const* streams);
+/* gub_p2p_step_keys_local_all with a Store plugin (see gub_submit_keys_store_async for the rule and gub_store_rec).  The step, its
+ * responses and the tables are those of gub_p2p_step_keys_local_all on the same input, except where Store.Get returned an item.  Every
+ * owner applies the single-table rule, per distinct key, to its pass: what it evaluates in the step, in source-rank order, then
+ * source-index order.  A record names its requests by source: `first` indexes shard first_shard's ingest batch (d_packed[first_shard]),
+ * `last` shard last_shard's.
+ *   get       called once per owner that has misses, in rank order, on the calling thread, with that owner's misses ordered by pass
+ *             index; every call completes before any owner installs or evaluates anything.  With a get the call BLOCKS until every
+ *             shard's routing of this step is done; get == NULL: as asynchronous as gub_p2p_step_keys_local_all.  A non-zero return
+ *             fails the call (the owners after it are not asked): no table is changed on any shard and d_out is undefined, but the
+ *             ring stays in step (every owner publishes its response flags without evaluating, every shard's epoch advances) and the
+ *             next step works normally.  The library keeps its own copy of each miss's request names (first, last, first_shard,
+ *             last_shard) and keys: what the callback writes there is ignored.
+ *             A table that cannot take the items Get returned fails the call the same way (nothing is evaluated, the ring stays in
+ *             step), but it is detected only after every owner has installed: each owner's table keeps the items it placed and the
+ *             parked inserts that were placed before them, as gub_add_items would have left it.
+ *   changes[r] / n_changes[r]   owner r's change log: page-locked (gub_host_alloc), room for world x cap records; valid once
+ *             streams[r] has completed the step.  Ordered by pass index; call Remove, then OnChange, for each record in turn.
+ * Refused (with text in gub_last_error()): GUB_PATH=fused; a ring with GLOBAL enabled (the owner-side application of a tick's hits
+ * would call Store.OnChange and needs a change log of its own); shards not connected with gub_p2p_connect_local; world x cap larger
+ * than an owner's pass (the table's max_batch after gub_p2p_create: one pass per step keeps one record per key); change logs outside
+ * page-locked memory.
+ * Memory, allocated by the first Store step: on every shard the table's Store scratch (as gub_submit_keys_store_async allocates it:
+ * 117 B x max_batch + 32 B x next_pow2(2 x max_batch) on the device, 200 B x max_batch page-locked) and an inverse map of its
+ * routing, 2 x world x cap x 4 B on the device, which the owners read over peer access. */
+int gub_p2p_step_keys_store_local_all(gub_p2p* const* ps, uint32_t world, const void* const* d_packed, const size_t* packed_bytes,
+                                      const size_t* n, const gub_params* params, size_t n_params, int64_t created_base,
+                                      const gub_clock* clk, gub_store_get_fn get, void* user, gub_resp* const* d_out,
+                                      gub_store_rec* const* changes, uint32_t* const* n_changes, void* const* streams);
 /* Device-side waits are bounded (a dead peer must not hang the GPU); a wait that gave up marks the step: *error_out != 0 and the
  * call fails with text in gub_last_error().  Requests whose owner never answered carry GUB_ERR_PEER_TIMEOUT in-band.  Costs a
  * device synchronisation: poll at your own cadence. */
