@@ -233,6 +233,13 @@ __device__ __forceinline__ void apply_invalid_at(const InvIndex& I, Bucket& b, b
   }
 }
 
+// Slots past home whose (w0, w1) pairs one probe round loads at once.  A lookup walks slots home, home + 1, ... (mod capacity) and
+// stops at the key, at the first EMPTY or after MAX_PROBE slots; at load factor 0.5 a quarter of the lookups need more than the home
+// slot and the longest lookup of a 22 k-key batch about 25 slots (DESIGN.md, "The table probe in rounds").  Loading one slot after the
+// other made that a chain of dependent round trips that the whole batch waits for; a round puts PROBE_ROUND independent 16-byte loads
+// in flight instead.  4, not 8: rounds of 8 made k_rank spill.
+constexpr int PROBE_ROUND = 4;
+
 // Looks `key` up.  On a hit the slot is loaded into cur.b.  On a miss cur.b is an empty (not live) bucket and cur.slot
 // is the first reusable slot (tombstone or empty) seen, if any.
 // (The home slot's four words arrive in a..d: callers that know the key early issue that load ahead of other work.)
@@ -240,17 +247,40 @@ __device__ __forceinline__ void cursor_open_preloaded(Cursor& cur, const Slot* t
                                                       ulonglong2 c, ulonglong2 d) {
   uint64_t idx = __umul64hi(key, cap);
   cur.home = idx; cur.found = false; cur.slot = -1;
+  bool hit = a.x == key && (a.y >> 8) == tag;
+  if (!hit && a.x == KEY_EMPTY) cur.slot = (int64_t)idx;
+  if (!hit && a.x != KEY_EMPTY) {
+    if (a.x == KEY_TOMB) cur.slot = (int64_t)idx;
+    bool done = false;
 #pragma unroll 1
-  for (int p = 0; p < MAX_PROBE; p++) {
-    if (p > 0) slot_load(table + idx, a, b, c, d);
-    if (a.x == key && (a.y >> 8) == tag) {
-      bucket_from(cur.b, a, b, c, d);
-      cur.old = cur.b; cur.slot = (int64_t)idx; cur.found = true;
-      return;
+    for (int p = 1; p < MAX_PROBE && !done; p += PROBE_ROUND) {
+      // every index wraps by itself: a table may be smaller than one round (the slots past the window are loaded, never examined)
+      ulonglong2 w[PROBE_ROUND];
+      uint64_t j = idx;
+#pragma unroll
+      for (int r = 0; r < PROBE_ROUND; r++) {
+        j = (j + 1 == cap) ? 0 : j + 1;
+        w[r] = __ldcg(reinterpret_cast<const ulonglong2*>(table + j));
+      }
+      // the same rules as for the home slot, in probe order
+#pragma unroll
+      for (int r = 0; r < PROBE_ROUND; r++) {
+        if (p + r >= MAX_PROBE) { done = true; break; }
+        idx = (idx + 1 == cap) ? 0 : idx + 1;
+        if (w[r].x == key && (w[r].y >> 8) == tag) { a = w[r]; hit = true; done = true; break; }
+        if (w[r].x == KEY_EMPTY) { if (cur.slot < 0) cur.slot = (int64_t)idx; done = true; break; }
+        if (w[r].x == KEY_TOMB && cur.slot < 0) cur.slot = (int64_t)idx;
+      }
     }
-    if (a.x == KEY_EMPTY) { if (cur.slot < 0) cur.slot = (int64_t)idx; break; }
-    if (a.x == KEY_TOMB && cur.slot < 0) cur.slot = (int64_t)idx;
-    idx = (idx + 1 == cap) ? 0 : idx + 1;
+    if (hit) {  // the rest of the slot: its first sector came with the pair, so this mostly hits L2
+      const ulonglong2* s = reinterpret_cast<const ulonglong2*>(table + idx);
+      b = __ldcg(s + 1); c = __ldcg(s + 2); d = __ldcg(s + 3);
+    }
+  }
+  if (hit) {
+    bucket_from(cur.b, a, b, c, d);
+    cur.old = cur.b; cur.slot = (int64_t)idx; cur.found = true;
+    return;
   }
   cur.b.key = key; cur.b.tag = tag; cur.b.flags = 0; cur.b.limit = 0; cur.b.duration = 0; cur.b.rem = 0; cur.b.stamp = 0;
   cur.b.burst = 0; cur.b.expire = 0;
