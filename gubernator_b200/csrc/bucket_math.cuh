@@ -60,6 +60,7 @@ enum : uint32_t {
   F_OVER = 2u,   // TokenBucketItem.Status == OVER_LIMIT (sticky, :168)
   F_LIVE = 4u,   // the cache holds an item for this key
   F_INVALID_AT = 8u,  // CacheItem.InvalidAt != 0 (set by Store / Loader plugins only): the value lives in the table's side index
+  F_STALE = 16u,      // InvalidAt < now, found when the slot was opened; never stored in the table (cursor_close drops it)
 };
 
 struct Bucket {
@@ -123,7 +124,9 @@ GUB_HD gub_resp apply_one(Bucket& b, const gub_req& rq, const gub_clock& clk, De
   const bool drain = (beh & GUB_BEHAVIOR_DRAIN_OVER_LIMIT) != 0;
   const int64_t hits = rq.hits, limit = rq.limit, created = rq.created_at;
 
-  // GetItem: an expired entry is removed and reported as a miss (lrucache.go:115-119; strict '<', cache.go:52)
+  // GetItem: an entry past its InvalidAt or its ExpireAt is removed and reported as a miss (cache.go:43-57, lrucache.go:115-119;
+  // strict '<').  Only here, after the algorithm check: a rejected request never reaches the cache (workers.go:317-320).
+  if (b.flags & F_STALE) b.flags &= ~(F_LIVE | F_INVALID_AT | F_STALE);
   if ((b.flags & F_LIVE) && b.expire < clk.now_ms) b.flags &= ~F_LIVE;
   bool have = (b.flags & F_LIVE) != 0;
   if (have) d.hit++; else d.miss++;

@@ -224,12 +224,12 @@ __device__ __forceinline__ void inv_store(const InvIndex& I, uint64_t key, uint6
   }
   I.e[home].key = key; I.e[home].tag = tag; I.e[home].invalid_at = invalid_at;
 }
-// IsExpired's first clause: an item past its InvalidAt counts as expired (removed, reported as a miss; the caller's apply_one sees a
-// bucket that is not live).
+// IsExpired's first clause: an item past its InvalidAt counts as expired.  The bucket is marked F_STALE; the first request that
+// reaches the cache (apply_one, past the algorithm check) removes it and reports a miss, one with a rejected algorithm leaves it.
 __device__ __forceinline__ void apply_invalid_at(const InvIndex& I, Bucket& b, bool found, int64_t now_ms) {
   if (found && (b.flags & F_INVALID_AT)) {
     const int64_t inv = inv_lookup(I, b.key, b.tag);
-    if (inv != 0 && inv < now_ms) b.flags &= ~(F_LIVE | F_INVALID_AT);
+    if (inv != 0 && inv < now_ms) b.flags |= F_STALE;
   }
 }
 
@@ -295,10 +295,11 @@ __device__ __forceinline__ void cursor_open(Cursor& cur, const Slot* table, uint
 // Writes cur.b back.  Returns false when a new key needed a slot and the probe window had none (table full).
 __device__ __forceinline__ bool cursor_close(Cursor& cur, Slot* table, uint64_t cap, uint32_t& inserts) {
   const Bucket& b = cur.b;
-  const uint64_t w1 = (b.tag << 8) | (uint64_t)(b.flags & 0xFF);
+  const uint32_t flags = b.flags & ~(uint32_t)F_STALE;  // (a mark of this batch, not slot state)
+  const uint64_t w1 = (b.tag << 8) | (uint64_t)(flags & 0xFF);
   if (cur.found) {
     ulonglong2* p = reinterpret_cast<ulonglong2*>(table + cur.slot);
-    if (b.flags != cur.old.flags) __stcg(p, make_ulonglong2(b.key, w1));
+    if (flags != (cur.old.flags & ~(uint32_t)F_STALE)) __stcg(p, make_ulonglong2(b.key, w1));
     if (b.limit != cur.old.limit || b.duration != cur.old.duration) __stcg(p + 1, make_ulonglong2((uint64_t)b.limit, (uint64_t)b.duration));
     if (b.rem != cur.old.rem || b.stamp != cur.old.stamp) __stcg(p + 2, make_ulonglong2(b.rem, (uint64_t)b.stamp));
     if (b.burst != cur.old.burst || b.expire != cur.old.expire) __stcg(p + 3, make_ulonglong2((uint64_t)b.burst, (uint64_t)b.expire));

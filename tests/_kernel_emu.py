@@ -39,6 +39,8 @@ def lib():
         L.emu_submit_compact.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, i64, vp, vp]
         L.emu_counters.argtypes = [vp, vp]; L.emu_counters.restype = None
         L.emu_scan.argtypes = [vp, vp, u64]; L.emu_scan.restype = u64
+        L.emu_add_items.argtypes = [vp, vp, u32]; L.emu_add_items.restype = u32
+        L.emu_get_items.argtypes = [vp, vp, vp, u32, i64, vp, vp]; L.emu_get_items.restype = None
         L.emu_sweep.argtypes = [vp, i64]; L.emu_sweep.restype = u64
         L.emu_sweep_range.argtypes = [vp, u64, u64, i64]; L.emu_sweep_range.restype = u64
         L.emu_random_rmw.argtypes = [vp, u64]; L.emu_random_rmw.restype = None
@@ -99,6 +101,18 @@ class EmuTable:
         out = np.zeros(self.capacity, dtype=item_dtype)
         n = self._L.emu_scan(self._h, out.ctypes.data, len(out))
         return out[:n]
+
+    def add_items(self, items):
+        items = np.ascontiguousarray(items)
+        assert items.dtype.itemsize == 88
+        assert self._L.emu_add_items(self._h, items.ctypes.data, len(items)) == 0, "table full"
+
+    def get_items(self, key_xxh64, key_fnv1, now_ms, item_dtype):
+        kx = np.ascontiguousarray(key_xxh64, dtype=np.uint64)
+        kf = np.ascontiguousarray(key_fnv1, dtype=np.uint64)
+        out, found = np.zeros(len(kx), dtype=item_dtype), np.zeros(len(kx), dtype=np.uint8)
+        self._L.emu_get_items(self._h, kx.ctypes.data, kf.ctypes.data, len(kx), int(now_ms), out.ctypes.data, found.ctypes.data)
+        return out, found.astype(bool)
 
     def sweep(self, now_ms):
         return int(self._L.emu_sweep(self._h, int(now_ms)))

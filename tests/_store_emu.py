@@ -9,6 +9,7 @@ import subprocess
 import numpy as np
 
 import _kernel_emu as E
+import edge_states as ES
 import oracle_py as O
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -85,29 +86,13 @@ class StoreTable(E.EmuTable):
 
 # ---- the host layer's rule (csrc/host_v1.cpp submit_with_store) over the oracle -------------------------------------------------------
 def oracle_to_item(it, kx, kf):
-    """An oracle CacheItem as gub_get_items reports it: token buckets carry no burst / float remaining, leaky ones no status / int remaining."""
-    r = np.zeros(1, dtype=ITEM_DTYPE)[0]
-    leaky = it.value_kind == 2
-    r["key_xxh64"], r["key_fnv1"] = kx, kf
-    r["algorithm"] = 1 if leaky else 0
-    r["status"] = 0 if leaky else it.status
-    r["limit"], r["duration"], r["stamp"], r["expire_at"], r["invalid_at"] = it.limit, it.duration, it.stamp, it.expire_at, it.invalid_at
-    r["remaining"] = 0 if leaky else it.remaining_i
-    r["remaining_f"] = it.remaining_f if leaky else 0.0
-    r["burst"] = it.burst if leaky else 0
-    return r
+    """An oracle CacheItem as gub_get_items reports it (bit for bit, NaN payloads included)."""
+    return ES.item_of_oracle(it, kx, kf)
 
 
 def item_to_oracle(r):
     """A gub_item as gub_add_items installs it (to_dev of gub_api.cu), as an oracle CacheItem."""
-    it = O.Item()
-    leaky = int(r["algorithm"]) == 1
-    it.algorithm = int(r["algorithm"]); it.value_kind = 2 if leaky else 1
-    it.expire_at = int(r["expire_at"]); it.invalid_at = int(r["invalid_at"])
-    it.status = 0 if leaky else int(r["status"]); it.limit = int(r["limit"]); it.duration = int(r["duration"])
-    it.remaining_i = 0 if leaky else int(r["remaining"]); it.remaining_f = float(r["remaining_f"]) if leaky else 0.0
-    it.stamp = int(r["stamp"]); it.burst = int(r["burst"]) if leaky else 0
-    return it
+    return ES.oracle_item(r)
 
 
 def model_batch(pool, reqs, now, store_items):
@@ -160,9 +145,18 @@ def model_batch(pool, reqs, now, store_items):
     return np.array(misses, dtype=REC_DTYPE), resp, np.array(recs, dtype=REC_DTYPE)
 
 
+_EDGE = ES.items()
+
+
 def store_item(rng, now, kind):
     """An item a Store could hold: 'token' / 'leaky' (live), 'expired', 'invalid' (past InvalidAt), 'pending' (InvalidAt ahead), 'bad'
-    (an algorithm the cache cannot hold)."""
+    (an algorithm the cache cannot hold), 'edge' (a state of edge_states.py, its times moved from edge_states.NOW to `now`)."""
+    if kind == "edge":
+        r = _EDGE[int(rng.integers(0, len(_EDGE)))].copy()
+        for f in ("stamp", "expire_at", "invalid_at"):
+            if r[f] not in (0, ES.I64_MIN, ES.I64_MAX):
+                r[f] = ES.wrap(int(r[f]) + now - ES.NOW)
+        return r
     r = np.zeros(1, dtype=ITEM_DTYPE)[0]
     leaky = kind == "leaky" or (kind not in ("token",) and rng.random() < 0.5)
     r["algorithm"] = 1 if leaky else 0
@@ -184,7 +178,7 @@ def store_item(rng, now, kind):
     return r
 
 
-def fill_store(rng, reqs, now, frac=0.3, kinds=("token", "leaky", "expired", "invalid", "pending", "bad")):
+def fill_store(rng, reqs, now, frac=0.3, kinds=("token", "leaky", "expired", "invalid", "pending", "bad", "edge")):
     """Store items for about `frac` of the batch's keys, of every kind."""
     out = {}
     for kx, kf in set(zip(reqs["key_xxh64"].tolist(), reqs["key_fnv1"].tolist())):

@@ -19,32 +19,6 @@ std::mutex g_emu_mu;  // the fiber scheduler has one global state: one emulated 
 thread_local std::string g_err;
 int fail(const std::string& m) { g_err = m; return -1; }
 
-DevItem to_dev(const gub_item& it) {  // same mapping as gub_api.cu
-  DevItem d;
-  std::memset(&d, 0, sizeof d);
-  d.key = it.key_xxh64 < 2 ? it.key_xxh64 + 2 : it.key_xxh64;
-  d.tag = it.key_fnv1 >> 8;
-  const bool leaky = it.algorithm == GUB_LEAKY_BUCKET;
-  d.flags = F_LIVE | (leaky ? F_LEAKY : 0u) | ((!leaky && it.status == GUB_OVER_LIMIT) ? F_OVER : 0u);
-  d.w[0] = (uint64_t)it.limit; d.w[1] = (uint64_t)it.duration;
-  if (leaky) std::memcpy(&d.w[2], &it.remaining_f, 8); else d.w[2] = (uint64_t)it.remaining;
-  d.w[3] = (uint64_t)it.stamp; d.w[4] = leaky ? (uint64_t)it.burst : 0; d.w[5] = (uint64_t)it.expire_at;
-  d.invalid_at = it.invalid_at;
-  return d;
-}
-gub_item from_dev(const DevItem& d) {
-  gub_item it;
-  std::memset(&it, 0, sizeof it);
-  it.key_xxh64 = d.key; it.key_fnv1 = d.tag << 8;
-  const bool leaky = (d.flags & F_LEAKY) != 0;
-  it.algorithm = leaky ? GUB_LEAKY_BUCKET : GUB_TOKEN_BUCKET;
-  it.status = (d.flags & F_OVER) ? GUB_OVER_LIMIT : GUB_UNDER_LIMIT;
-  it.limit = (int64_t)d.w[0]; it.duration = (int64_t)d.w[1];
-  if (leaky) std::memcpy(&it.remaining_f, &d.w[2], 8); else it.remaining = (int64_t)d.w[2];
-  it.stamp = (int64_t)d.w[3]; it.burst = (int64_t)d.w[4]; it.expire_at = (int64_t)d.w[5];
-  it.invalid_at = d.invalid_at;
-  return it;
-}
 }  // namespace
 
 extern "C" {

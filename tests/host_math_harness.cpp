@@ -83,4 +83,17 @@ int hm_rank_check(const Bucket* b0, const gub_req* rq, uint32_t m, const gub_clo
 }
 
 size_t hm_sizeof_bucket() { return sizeof(Bucket); }
+
+// Element-wise entries over arrays; tests/bucket_math_dev.cu exports the same signatures over the device build of the header.
+void hm_f2i(const double* x, int64_t* out, size_t n) {
+  for (size_t i = 0; i < n; i++) out[i] = f2i(x[i]);
+}
+// b[i] <- apply_one(b[i], rq[i]); d[i] holds that one application's counter deltas
+void hm_apply_one(Bucket* b, const gub_req* rq, const gub_clock* clk, size_t n, gub_resp* out, Delta* d) {
+  for (size_t i = 0; i < n; i++) { d[i] = Delta{0, 0, 0}; out[i] = apply_one(b[i], rq[i], *clk, d[i]); }
+}
+// b[i] <- the state after rank target[i] of a run of identical requests rq[i]
+void hm_run_to_rank(Bucket* b, const gub_req* rq, const uint32_t* target, const gub_clock* clk, size_t n, gub_resp* out, Delta* d) {
+  for (size_t i = 0; i < n; i++) { d[i] = Delta{0, 0, 0}; out[i] = run_to_rank(b[i], rq[i], target[i], *clk, d[i]); }
+}
 }

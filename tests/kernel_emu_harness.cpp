@@ -52,6 +52,32 @@ struct EmuTable {  // what gub_create allocates (gub_api.cu), one scratch set
 
 uint32_t g_fused = 0;  // emu_set_fused(1): the persistent kernel k_batch instead of the four-kernel pipeline (single tables and rings alike)
 
+DevItem to_dev(const gub_item& it) {  // same mapping as gub_api.cu
+  DevItem d;
+  std::memset(&d, 0, sizeof d);
+  d.key = it.key_xxh64 < 2 ? it.key_xxh64 + 2 : it.key_xxh64;
+  d.tag = it.key_fnv1 >> 8;
+  const bool leaky = it.algorithm == GUB_LEAKY_BUCKET;
+  d.flags = F_LIVE | (leaky ? F_LEAKY : 0u) | ((!leaky && it.status == GUB_OVER_LIMIT) ? F_OVER : 0u);
+  d.w[0] = (uint64_t)it.limit; d.w[1] = (uint64_t)it.duration;
+  if (leaky) std::memcpy(&d.w[2], &it.remaining_f, 8); else d.w[2] = (uint64_t)it.remaining;
+  d.w[3] = (uint64_t)it.stamp; d.w[4] = leaky ? (uint64_t)it.burst : 0; d.w[5] = (uint64_t)it.expire_at;
+  d.invalid_at = it.invalid_at;
+  return d;
+}
+gub_item from_dev(const DevItem& d) {
+  gub_item it;
+  std::memset(&it, 0, sizeof it);
+  it.key_xxh64 = d.key; it.key_fnv1 = d.tag << 8;
+  const bool leaky = (d.flags & F_LEAKY) != 0;
+  it.algorithm = leaky ? GUB_LEAKY_BUCKET : GUB_TOKEN_BUCKET;
+  it.status = (d.flags & F_OVER) ? GUB_OVER_LIMIT : GUB_UNDER_LIMIT;
+  it.limit = (int64_t)d.w[0]; it.duration = (int64_t)d.w[1];
+  if (leaky) std::memcpy(&it.remaining_f, &d.w[2], 8); else it.remaining = (int64_t)d.w[2];
+  it.stamp = (int64_t)d.w[3]; it.burst = (int64_t)d.w[4]; it.expire_at = (int64_t)d.w[5];
+  it.invalid_at = d.invalid_at;
+  return it;
+}
 }  // namespace
 
 extern "C" {
@@ -212,20 +238,28 @@ uint64_t emu_scan(void* tv, gub_item* out, uint64_t cap) {
   unsigned long long n = 0;
   emu::launch(k_scan, 4u, 256u, (const Slot*)t->table, t->capacity, dev.data(), (unsigned long long)cap, &n, t->inv);
   const uint64_t m = std::min<uint64_t>(n, cap);
-  for (uint64_t i = 0; i < m; i++) {
-    const DevItem& d = dev[i];
-    gub_item it;
-    std::memset(&it, 0, sizeof it);
-    it.key_xxh64 = d.key; it.key_fnv1 = d.tag << 8;
-    const bool leaky = (d.flags & F_LEAKY) != 0;
-    it.algorithm = leaky ? GUB_LEAKY_BUCKET : GUB_TOKEN_BUCKET;
-    it.status = (d.flags & F_OVER) ? GUB_OVER_LIMIT : GUB_UNDER_LIMIT;
-    it.limit = (int64_t)d.w[0]; it.duration = (int64_t)d.w[1];
-    if (leaky) std::memcpy(&it.remaining_f, &d.w[2], 8); else it.remaining = (int64_t)d.w[2];
-    it.stamp = (int64_t)d.w[3]; it.burst = (int64_t)d.w[4]; it.expire_at = (int64_t)d.w[5]; it.invalid_at = d.invalid_at;
-    out[i] = it;
-  }
+  for (uint64_t i = 0; i < m; i++) out[i] = from_dev(dev[i]);
   return n;
+}
+
+// gub_add_items / gub_get_items of gub_api.cu (k_add_items / k_get_items and the gub_item <-> DevItem mapping); duplicate keys in
+// one call are not merged here, callers pass distinct keys.
+uint32_t emu_add_items(void* tv, const gub_item* items, uint32_t n) {
+  EmuTable* t = static_cast<EmuTable*>(tv);
+  std::vector<DevItem> dev;
+  for (uint32_t i = 0; i < n; i++)
+    if (items[i].algorithm == GUB_TOKEN_BUCKET || items[i].algorithm == GUB_LEAKY_BUCKET) dev.push_back(to_dev(items[i]));
+  uint32_t failed = 0;
+  if (!dev.empty())
+    emu::launch(k_add_items, (unsigned)((dev.size() + 255) / 256), 256u, t->table, t->capacity, (const DevItem*)dev.data(), (uint32_t)dev.size(),
+                t->counters, &failed, t->inv);
+  return failed;
+}
+void emu_get_items(void* tv, const uint64_t* kx, const uint64_t* kf, uint32_t n, int64_t now_ms, gub_item* out, uint8_t* found) {
+  EmuTable* t = static_cast<EmuTable*>(tv);
+  std::vector<DevItem> host(std::max<uint32_t>(n, 1));
+  if (n) emu::launch(k_get_items, (n + 255) / 256, 256u, (const Slot*)t->table, t->capacity, kx, kf, n, now_ms, host.data(), found, t->inv);
+  for (uint32_t i = 0; i < n; i++) { out[i] = from_dev(host[i]); out[i].key_xxh64 = kx[i]; out[i].key_fnv1 = kf[i]; }
 }
 
 // gub_probe_random_access's kernel (the timing around it is host code): the table must come out unchanged.

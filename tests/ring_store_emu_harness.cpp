@@ -103,7 +103,7 @@ int emu_ring_store_step(void* pv, const gub_req* const* reqs, const uint32_t* n,
         rr.first = named[k].first; rr.last = named[k].last; rr.first_shard = named[k].first_shard; rr.last_shard = named[k].last_shard;
         rr.item.key_xxh64 = named[k].item.key_xxh64; rr.item.key_fnv1 = named[k].item.key_fnv1;
         loaded[r].push_back(make_uint4(rr.first, rr.item.expire_at >= clk->now_ms ? S_EXISTED : 0u, (uint32_t)rr.item.algorithm, (uint32_t)rr.first_shard));
-        if (rr.item.algorithm == GUB_TOKEN_BUCKET || rr.item.algorithm == GUB_LEAKY_BUCKET) items[r].push_back(item_dev(rr.item));
+        if (rr.item.algorithm == GUB_TOKEN_BUCKET || rr.item.algorithm == GUB_LEAKY_BUCKET) items[r].push_back(to_dev(rr.item));
       }
     }
     for (uint32_t r = 0; r < W && rc == 0; r++) {

@@ -20,20 +20,6 @@ struct EmuStore {
 };
 std::map<void*, EmuStore> g_store;
 
-DevItem item_dev(const gub_item& it) {  // to_dev of gub_api.cu
-  DevItem d;
-  std::memset(&d, 0, sizeof d);
-  d.key = it.key_xxh64 < 2 ? it.key_xxh64 + 2 : it.key_xxh64;
-  d.tag = it.key_fnv1 >> 8;
-  const bool leaky = it.algorithm == GUB_LEAKY_BUCKET;
-  d.flags = F_LIVE | (leaky ? F_LEAKY : 0u) | ((!leaky && it.status == GUB_OVER_LIMIT) ? F_OVER : 0u);
-  d.w[0] = (uint64_t)it.limit; d.w[1] = (uint64_t)it.duration;
-  if (leaky) std::memcpy(&d.w[2], &it.remaining_f, 8); else d.w[2] = (uint64_t)it.remaining;
-  d.w[3] = (uint64_t)it.stamp; d.w[4] = leaky ? (uint64_t)it.burst : 0; d.w[5] = (uint64_t)it.expire_at;
-  d.invalid_at = it.invalid_at;
-  return d;
-}
-
 }  // namespace
 
 extern "C" {
@@ -99,7 +85,7 @@ int emu_store_submit(void* tv, const gub_req* reqs, size_t n, const gub_clock* c
         if (!(r.flags & GUB_STORE_FOUND)) continue;
         r.item.key_xxh64 = keys[2 * k]; r.item.key_fnv1 = keys[2 * k + 1];
         loaded.push_back(make_uint4(r.first, r.item.expire_at >= clk->now_ms ? S_EXISTED : 0u, (uint32_t)r.item.algorithm, 0u));
-        if (r.item.algorithm == GUB_TOKEN_BUCKET || r.item.algorithm == GUB_LEAKY_BUCKET) items.push_back(item_dev(r.item));
+        if (r.item.algorithm == GUB_TOKEN_BUCKET || r.item.algorithm == GUB_LEAKY_BUCKET) items.push_back(to_dev(r.item));
       }
       if (!items.empty()) {
         gub_clock dclk;

@@ -147,7 +147,9 @@ def calls_of(st, recs):
         if rec["flags"] & S.STORE_REMOVE:
             out.append(("Remove", key))
         if rec["flags"] & S.STORE_CHANGE:
-            out.append(("OnChange", key, tuple(rec["item"][f].item() for f in ITEM_FIELDS)))
+            # remaining_f as its bits: a Store may hand back NaNs, which never compare equal as floats
+            out.append(("OnChange", key, tuple(int(np.float64(rec["item"][f]).view(np.uint64)) if f == "remaining_f" else rec["item"][f].item()
+                                               for f in ITEM_FIELDS)))
     return out
 
 

@@ -34,7 +34,8 @@ class MockStore:
         return self.items.get(key)
 
     def on_change(self, req, key, item):
-        self.calls.append(("OnChange", key, item))
+        # remaining_f as its bits: a Store may hold NaNs (edge items), which never compare equal as floats
+        self.calls.append(("OnChange", key, dict(item, remaining_f=int(np.float64(item["remaining_f"]).view(np.uint64)))))
 
     def remove(self, key):
         self.calls.append(("Remove", key))
@@ -176,7 +177,7 @@ def _store_items(rng, kb, now, frac=0.35):
     items = {}
     for k in sorted(set(kb.keys)):
         if rng.random() < frac:
-            kind = ("token", "leaky", "expired")[int(rng.integers(0, 3))]
+            kind = ("token", "leaky", "expired", "edge")[int(rng.integers(0, 4))]  # (this item dict carries no InvalidAt)
             r = S.store_item(rng, now, kind)
             items[k.decode()] = {f: (float(r[f]) if f == "remaining_f" else int(r[f])) for f in ITEM_FIELDS}
     return items

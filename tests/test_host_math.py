@@ -3,8 +3,9 @@ apply_one() against the oracle, and plan_run()/eval_piece() against repeated app
 import numpy as np
 import pytest
 
+import edge_states as ES
 import oracle_py as O
-from _host_math import BUCKET_DTYPE, F_LEAKY, F_LIVE, F_OVER, HostTable, plan_check, rank_check
+from _host_math import BUCKET_DTYPE, F_LEAKY, F_LIVE, F_OVER, HostTable, apply_one, lib, plan_check, rank_check
 from workloads import T0, adversarial_batch, bench_batch, extreme_batch, make_clock
 
 
@@ -44,7 +45,12 @@ def test_apply_one_matches_oracle_bench_traffic():
         _cmp(host.apply_seq(reqs, make_clock(now))[0], pool.submit_hashed(reqs))
 
 
+_EDGE = ES.buckets(BUCKET_DTYPE)
+
+
 def _rand_bucket(rng, now):
+    if rng.random() < 0.25:  # a state only a Store or Loader installs (edge_states.py)
+        return _EDGE[int(rng.integers(0, len(_EDGE)))][None].copy()
     b = np.zeros(1, dtype=BUCKET_DTYPE)
     leaky = rng.random() < 0.5
     b["flags"] = (F_LIVE if rng.random() < 0.9 else 0) | (F_LEAKY if leaky else 0) | (F_OVER if (not leaky and rng.random() < 0.2) else 0)
@@ -119,3 +125,35 @@ def test_apply_one_matches_oracle_on_numeric_extremes(seed):
         _cmp(got, want)
         oc = pool.counters()
         assert (ctr["over_limit"], ctr["cache_hit"], ctr["cache_miss"]) == (oc["over_limit"], oc["cache_hit"], oc["cache_miss"])
+
+
+def _check_loaded_state(b, it, what):
+    """A slot image after apply_one against the oracle's CacheItem for the same key, bit for bit."""
+    assert (int(b["limit"]), int(b["duration"]), int(b["stamp"]), int(b["expire"])) == (it.limit, it.duration, it.stamp, it.expire_at), what
+    if it.value_kind == 2:
+        assert int(b["flags"]) & F_LEAKY and int(b["burst"]) == it.burst, what
+        assert int(b["rem"]) == ES.oracle_rem_bits(it), (what, hex(int(b["rem"])), hex(ES.oracle_rem_bits(it)))
+    else:
+        assert not int(b["flags"]) & F_LEAKY and int(b["rem"]) == it.remaining_i % (1 << 64) and bool(int(b["flags"]) & F_OVER) == (it.status == 1), what
+
+
+@pytest.mark.parametrize("seed", range(2))
+def test_apply_one_matches_oracle_on_loaded_states(seed):
+    """Every lattice state of edge_states.py, loaded into the oracle bit for bit, under requests drawn around it: one apply_one()
+    per (state, request) pair gives the oracle's response, counters and stored item."""
+    rng = np.random.default_rng(7100 + seed)
+    b, rq, _, idx = ES.pairs(rng, 40000, BUCKET_DTYPE, O.HREQ_DTYPE)
+    its = ES.items()
+    pool = O.Pool(workers=4, cache_size=10_000_000, now_ms=ES.NOW)
+    for i in range(len(rq)):
+        pool.add_item_hashed(rq["key_xxh64"][i], rq["key_fnv1"][i], ES.oracle_item(its[idx[i]]))
+    clk = make_clock(ES.NOW)
+    got, after, d = apply_one(lib(), b, rq, clk)
+    _cmp(got, pool.submit_hashed(rq))
+    oc = pool.counters()
+    assert (int(d["over"].sum()), int(d["hit"].sum()), int(d["miss"].sum())) == (oc["over_limit"], oc["cache_hit"], oc["cache_miss"])
+    held = pool.each()
+    live = (after["flags"] & F_LIVE) != 0
+    assert len(held) == int(live.sum())
+    for i in np.nonzero(live)[0]:
+        _check_loaded_state(after[i], held[(int(rq["key_xxh64"][i]), int(rq["key_fnv1"][i]))], (i, b[i], rq[i]))

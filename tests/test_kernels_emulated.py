@@ -7,6 +7,7 @@ no GPU, and lets a kernel change be tried before GPU minutes are spent on it."""
 import numpy as np
 import pytest
 
+import edge_states as ES
 import oracle_py as O
 import _kernel_emu as E
 from workloads import T0, adversarial_batch, bench_requests, extreme_batch, key_hashes, make_clock, zipf_ids
@@ -93,6 +94,34 @@ def test_numeric_extremes(G, path):
         reqs = extreme_batch(rng, 2000, 30, now)
         _cmp(tab.submit(reqs, make_clock(now), O.HRESP_DTYPE), pool.submit_hashed(reqs), f"step {step}")
     _check_state(G, tab, pool)
+
+
+@both_paths
+def test_loaded_states_match_oracle(G, path):
+    """Every state of edge_states.py installed with k_add_items (and into the oracle bit for bit), then its request plans: all
+    short plans on every state, the long uniform runs and the chunk-crossing and one-request-segment runs on every 16th.
+    Responses, counters, get_items and the scan (remaining_f as bits) equal the oracle's."""
+    its, plans = ES.lattice(O.HREQ_DTYPE, lambda i, j, p: len(p) <= 40 or i % 16 == 0)
+    tab, pool = Tab(path, 1 << 15), O.Pool(workers=4, cache_size=10_000_000, now_ms=ES.NOW)
+    tab.add_items(its)
+    for r in its:
+        pool.add_item_hashed(r["key_xxh64"], r["key_fnv1"], ES.oracle_item(r))
+    reqs = np.concatenate([plans[i] for i in np.random.default_rng(12).permutation(len(plans))])
+    for off in range(0, len(reqs), 65536):
+        chunk = np.ascontiguousarray(reqs[off:off + 65536])
+        _cmp(tab.submit(chunk, make_clock(ES.NOW), O.HRESP_DTYPE), pool.submit_hashed(chunk), f"batch at {off}")
+    c, oc = tab.counters(), pool.counters()
+    assert all(c[k] == oc[k] for k in ("over_limit", "cache_hit", "cache_miss")), (c, oc)
+    assert c["dup_groups"] > 0 and c["mixed_groups"] > 0 and c["serial_fallbacks"] > 0, c
+    scan, held = ES.keyed_scan(tab.scan(G.ITEM_DTYPE), pool.each())
+    assert scan.keys() == held.keys()
+    for k, it in held.items():
+        assert scan[k].tobytes() == ES.item_of_oracle(it, *k).tobytes(), ("scan", scan[k], ES.item_of_oracle(it, *k))
+    got, found = tab.get_items(its["key_xxh64"], its["key_fnv1"], ES.NOW, G.ITEM_DTYPE)  # after the scan: GetItem removes expired items
+    for i, r in enumerate(its):
+        it = pool.get_item_hashed(r["key_xxh64"], r["key_fnv1"])
+        assert found[i] == (it is not None), (i, r)
+        assert it is None or got[i].tobytes() == ES.item_of_oracle(it, r["key_xxh64"], r["key_fnv1"]).tobytes(), ("get_items", i, r, got[i])
 
 
 @both_paths
