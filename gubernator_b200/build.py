@@ -9,7 +9,7 @@ ROOT = os.path.dirname(HERE)
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libgubernator_b200.so")
 SOURCES = [os.path.join(CSRC, f) for f in ("gub_api.cu", "host_util.cpp", "host_v1.cpp")]
-DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("gub_kernels.cuh", "gub_batch.cuh", "gub_global.cuh", "gub_p2p.cuh", "gub_store.cuh", "bucket_math.cuh")] + \
+DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("gub_kernels.cuh", "gub_batch.cuh", "gub_global.cuh", "gub_p2p.cuh", "gub_store.cuh", "gub_proto.cuh", "bucket_math.cuh")] + \
     [os.path.join(ROOT, "include", f) for f in ("gubernator_b200.h", "gubernator_b200_host.h")]
 
 NVCC_FLAGS = [

@@ -22,6 +22,7 @@
 #include "gub_global.cuh"
 #include "gub_p2p.cuh"
 #include "gub_store.cuh"
+#include "gub_proto.cuh"
 
 extern "C" uint64_t gub_ring_version_(const gub_ring* r);
 
@@ -51,6 +52,17 @@ struct PipeSlot {
   size_t cap = 0, params_cap = 0;
   cudaEvent_t in_done = nullptr, out_done = nullptr;
   bool busy = false;
+  // wire-format submissions (gub_submit_proto_async): scratch sized by the call's input, grown on demand
+  struct Proto {
+    uint32_t *slot_base = nullptr, *batch_base = nullptr, *mcount = nullptr, *meval = nullptr, *mstatus = nullptr, *msize = nullptr;
+    unsigned long long* moff = nullptr;
+    gub::ProtoItem* items = nullptr;
+    gub_req* sreq = nullptr;
+    uint8_t *keys = nullptr, *stage = nullptr;
+    size_t msgs_cap = 0, slots_cap = 0, bytes_cap = 0;
+    uint32_t* h_neval = nullptr;      // mapped: the call's evaluable item count, written by k_proto_scan
+    cudaEvent_t decoded = nullptr;
+  } proto;
 };
 
 uint32_t next_pow2(uint64_t v) { uint64_t p = 1; while (p < v) p <<= 1; return (uint32_t)p; }
@@ -103,6 +115,7 @@ struct gub_table {
   bool last_pending = false;          // work was enqueued on last_stream after (or without) the last event record
   // host path
   cudaStream_t s_h2d = nullptr, s_compute = nullptr, s_d2h = nullptr;
+  cudaStream_t s_proto = nullptr;     // decoding of wire-format calls: touches no table, so it does not wait for earlier evaluations
   cudaEvent_t compute_done[PIPE_DEPTH] = {};
   PipeSlot pipe[PIPE_DEPTH];
   int next_slot = 0;
@@ -477,6 +490,11 @@ void gub_destroy(gub_table* t) {
     if (s.d_params) cudaFree(s.d_params);
     if (s.in_done) cudaEventDestroy(s.in_done);
     if (s.out_done) cudaEventDestroy(s.out_done);
+    auto& pr = s.proto;
+    void* dev[] = {pr.slot_base, pr.batch_base, pr.mcount, pr.meval, pr.mstatus, pr.msize, pr.moff, pr.items, pr.sreq, pr.keys, pr.stage};
+    for (void* p : dev) if (p) cudaFree(p);
+    if (pr.h_neval) cudaFreeHost(pr.h_neval);
+    if (pr.decoded) cudaEventDestroy(pr.decoded);
   }
   for (auto& e : t->compute_done) if (e) cudaEventDestroy(e);
   for (auto& e : t->prof_ev) cudaEventDestroy(e);
@@ -493,6 +511,7 @@ void gub_destroy(gub_table* t) {
   if (t->s_h2d) cudaStreamDestroy(t->s_h2d);
   if (t->s_compute) cudaStreamDestroy(t->s_compute);
   if (t->s_d2h) cudaStreamDestroy(t->s_d2h);
+  if (t->s_proto) cudaStreamDestroy(t->s_proto);
   delete t;
 }
 
@@ -924,6 +943,129 @@ int gub_submit_keys_store_async(gub_table* t, const void* packed, size_t packed_
   if (!sc.changes || !sc.n_changes) return fail("gub_submit_keys_store_async: changes and n_changes must be page-locked host memory (gub_host_alloc)");
   if (n == 0) *n_changes = 0;
   return submit_keys(t, packed, packed_bytes, n, params, n_params, created_base, clk, out, ticket, &sc);
+}
+
+int gub_proto_layout(size_t n_msgs, size_t msg_bytes, size_t* offsets_at, size_t* bytes_at, size_t* total, size_t* out_bound) {
+  if (!offsets_at || !bytes_at || !total || !out_bound) return fail("gub_proto_layout: null argument");
+  *offsets_at = n_msgs * 8;
+  *bytes_at = *offsets_at + (n_msgs + 1) * 4;
+  *total = (*bytes_at + msg_bytes + 15) & ~(size_t)15;
+  *out_bound = (size_t)gub::PROTO_OUT_FACTOR * msg_bytes;
+  return 0;
+}
+
+}  // extern "C"
+
+namespace {
+int proto_ensure(PipeSlot& s, const gub::ProtoPlan& P, size_t n_msgs) {
+  auto& pr = s.proto;
+  if (!pr.decoded) {
+    CK(cudaEventCreateWithFlags(&pr.decoded, cudaEventDisableTiming));
+    CK(cudaHostAlloc((void**)&pr.h_neval, 64, cudaHostAllocMapped));
+  }
+  if (pr.msgs_cap < n_msgs + 1) {
+    const size_t c = std::max<size_t>(n_msgs + 1, 1024);
+    uint32_t** u32s[] = {&pr.slot_base, &pr.batch_base, &pr.mcount, &pr.meval, &pr.mstatus, &pr.msize};
+    for (uint32_t** a : u32s) { if (*a) cudaFree(*a); *a = nullptr; CK(cudaMalloc(a, c * 4)); }
+    if (pr.moff) cudaFree(pr.moff);
+    pr.moff = nullptr;
+    CK(cudaMalloc(&pr.moff, c * 8));
+    pr.msgs_cap = c;
+  }
+  if (pr.slots_cap < P.slots || !pr.items) {
+    const size_t c = std::max<size_t>(P.slots + P.slots / 4, 1024);
+    if (pr.items) cudaFree(pr.items);
+    if (pr.sreq) cudaFree(pr.sreq);
+    pr.items = nullptr; pr.sreq = nullptr;
+    CK(cudaMalloc(&pr.items, c * sizeof(gub::ProtoItem)));
+    CK(cudaMalloc(&pr.sreq, c * sizeof(gub_req)));
+    pr.slots_cap = c;
+  }
+  if (pr.bytes_cap < P.msg_bytes || !pr.keys) {
+    const size_t c = std::max<size_t>(P.msg_bytes + P.msg_bytes / 4, (size_t)1 << 16);
+    if (pr.keys) cudaFree(pr.keys);
+    if (pr.stage) cudaFree(pr.stage);
+    pr.keys = nullptr; pr.stage = nullptr;
+    CK(cudaMalloc(&pr.keys, c));
+    CK(cudaMalloc(&pr.stage, c * gub::PROTO_OUT_FACTOR));
+    pr.bytes_cap = c;
+  }
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+/* Wire bytes in, wire bytes out (see the header).  Decoding runs on s_proto, which waits only for this call's copy; the host then waits
+ * for the decoded item count (a mapped word), so that the evaluation is sized for the items there are, and enqueues the evaluation and
+ * the encoding on the compute stream. */
+int gub_submit_proto_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n_msgs, const gub_clock* clk, void* out_bytes,
+                           size_t out_cap, uint64_t* out_off, uint32_t* msg_status, int* ticket) {
+  const std::string what = "gub_submit_proto_async";
+  if (!t || !clk || !ticket || !out_off || (n_msgs && (!packed || !out_bytes || !msg_status))) return fail(what + ": null argument");
+  if (n_msgs > 0x7FFFFFFFull) return fail(what + ": too many messages");
+  gub::ProtoPlan P;
+  if (n_msgs) {
+    if (const char* why = gub::proto_plan(static_cast<const uint8_t*>(packed), packed_bytes, n_msgs, out_cap, P)) return fail(what + ": " + why);
+  }
+  CK(cudaSetDevice(t->device));
+  uint8_t* d_out = n_msgs ? pinned_view(static_cast<uint8_t*>(out_bytes)) : nullptr;
+  unsigned long long* d_off = pinned_view(reinterpret_cast<unsigned long long*>(out_off));
+  uint32_t* d_status = n_msgs ? pinned_view(msg_status) : nullptr;
+  if (!d_off || (n_msgs && (!d_out || !d_status)))
+    return fail(what + ": out_bytes, out_off and msg_status must be page-locked host memory (gub_host_alloc)");
+  std::lock_guard<std::mutex> lk(t->mu);
+  const int si = t->next_slot;
+  t->next_slot = (t->next_slot + 1) % PIPE_DEPTH;
+  PipeSlot& s = t->pipe[si];
+  if (s.busy) { CK(cudaEventSynchronize(s.out_done)); s.busy = false; }
+  *ticket = si;
+  if (n_msgs == 0) { out_off[0] = 0; CK(cudaEventRecord(s.out_done, t->s_compute)); s.busy = true; return 0; }
+  if (!t->s_proto) {
+    CK(cudaStreamCreateWithFlags(&t->s_proto, cudaStreamNonBlocking));
+    CK(cudaFuncSetAttribute(gub::k_proto_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gub::PROTO_SMEM));
+  }
+  if (ensure_slot(s, std::max<size_t>(P.slots, 1)) || proto_ensure(s, P, n_msgs)) return -1;
+  if (s.packed_cap < packed_bytes) {
+    if (s.d_packed) cudaFree(s.d_packed);
+    s.d_packed = nullptr;
+    s.packed_cap = std::max<size_t>(packed_bytes + packed_bytes / 4, (size_t)1 << 20);
+    CK(cudaMalloc(&s.d_packed, s.packed_cap));
+  }
+  auto& pr = s.proto;
+  CK(cudaMemcpyAsync(s.d_packed, packed, P.bytes_at + P.msg_bytes, cudaMemcpyHostToDevice, t->s_h2d));
+  CK(cudaEventRecord(s.in_done, t->s_h2d));
+  CK(cudaStreamWaitEvent(t->s_proto, s.in_done, 0));
+  gub::ProtoArgs A;
+  std::memset(&A, 0, sizeof A);
+  A.created = reinterpret_cast<const int64_t*>(s.d_packed);
+  A.offs = reinterpret_cast<const uint32_t*>(s.d_packed + P.offsets_at);
+  A.bytes = s.d_packed + P.bytes_at;
+  A.n_msgs = (uint32_t)n_msgs;
+  A.smem = P.smem;
+  A.slot_base = pr.slot_base; A.batch_base = pr.batch_base; A.mcount = pr.mcount; A.meval = pr.meval; A.mstatus = pr.mstatus;
+  A.msize = pr.msize; A.moff = pr.moff; A.items = pr.items; A.sreq = pr.sreq; A.keys = pr.keys; A.stage = pr.stage;
+  A.reqs = s.d_req; A.resp = s.d_resp;
+  if (device_view(pr.h_neval, &A.n_eval)) return -1;
+  A.out = d_out; A.out_off = d_off; A.out_status = d_status;
+  const unsigned grid = (unsigned)n_msgs;
+  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, t->s_proto>>>(A, 0u);
+  gub::k_proto_decode<<<grid, gub::PROTO_THREADS, P.smem, t->s_proto>>>(A);
+  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, t->s_proto>>>(A, 1u);
+  gub::k_proto_compact<<<grid, gub::PROTO_THREADS, 0, t->s_proto>>>(A);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(pr.decoded, t->s_proto));
+  CK(cudaEventSynchronize(pr.decoded));
+  const uint32_t n_eval = *(volatile uint32_t*)pr.h_neval;
+  CK(cudaStreamWaitEvent(t->s_compute, pr.decoded, 0));
+  if (n_eval && launch_batch(t, s.d_req, n_eval, clk, s.d_resp, t->s_compute)) return -1;
+  gub::k_proto_encode<<<grid, gub::PROTO_THREADS, 0, t->s_compute>>>(A);
+  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, t->s_compute>>>(A, 2u);
+  gub::k_proto_copy_out<<<grid, gub::PROTO_THREADS, 0, t->s_compute>>>(A);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(s.out_done, t->s_compute));
+  s.busy = true;
+  return 0;
 }
 
 int gub_wait(gub_table* t, int ticket) {

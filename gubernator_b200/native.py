@@ -55,7 +55,7 @@ EXPORTS = ["gub_create", "gub_destroy", "gub_last_error", "gub_abi_version", "gu
            "gub_p2p_connect_local", "gub_p2p_step", "gub_p2p_step_streams", "gub_p2p_status", "gub_p2p_enable_global", "gub_nccl_unique_id",
            "gub_p2p_nccl_init", "gub_p2p_nccl_init_local", "gub_global_tick", "gub_gq_dropped", "gub_set_sweep", "gub_set_trace", "gub_get_trace", "gub_get_trace_raw", "gub_get_ktrace", "gub_keys_layout", "gub_submit_keys_async", "gub_global_tick_local_all", "gub_p2p_step_local_all",
            "gub_p2p_step_keys", "gub_p2p_step_keys_local_all", "gub_p2p_step_mixed_local_all",
-           "gub_submit_keys_store_async", "gub_p2p_step_keys_store_local_all"]
+           "gub_submit_keys_store_async", "gub_p2p_step_keys_store_local_all", "gub_proto_layout", "gub_submit_proto_async"]
 
 
 class Config(C.Structure):
@@ -157,6 +157,8 @@ _LATE_ARGTYPES = {
     "gub_p2p_step_mixed_local_all": [_pvp, C.c_uint32, _pvp, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, _pvp, _pvp],
     "gub_submit_keys_store_async": [_vp, _vp, _sz, _sz, _vp, _sz, C.c_int64, _vp, STORE_GET_FN, _vp, _vp, _vp, _vp, C.POINTER(C.c_int)],
     "gub_p2p_step_keys_store_local_all": [_pvp, C.c_uint32, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, STORE_GET_FN, _vp, _pvp, _pvp, _pvp, _pvp],
+    "gub_proto_layout": [_sz, _sz, _psz, _psz, _psz, _psz],
+    "gub_submit_proto_async": [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _vp, _vp, C.POINTER(C.c_int)],
 }
 
 
@@ -362,6 +364,16 @@ class Table:
                "gub_submit_keys_store_async")
         return tk.value
 
+    def submit_proto_async(self, packed_ptr, packed_bytes, n_msgs, clk, out_ptr, out_cap, out_off_ptr, status_ptr):
+        """GetRateLimitsReq wire bytes in (packed: see pack_proto), GetRateLimitsResp wire bytes out (gub_submit_proto_async).  out_ptr
+        (out_cap bytes, at least pack_proto's bound), out_off_ptr (n_msgs + 1 uint64) and status_ptr (n_msgs uint32) must be page-locked
+        (PinnedArray).  After wait(): message m's response is out[out_off[m]:out_off[m + 1]], its status PROTO_OK / PROTO_TOO_LARGE /
+        PROTO_MALFORMED.  Returns a ticket for wait()."""
+        tk = C.c_int(-1)
+        _check(_entry("gub_submit_proto_async")(self._h, packed_ptr, packed_bytes, n_msgs, clk.ctypes.data, out_ptr, out_cap, out_off_ptr, status_ptr,
+                                            C.byref(tk)), "gub_submit_proto_async")
+        return tk.value
+
     def set_sweep(self, slots_per_cta):
         _check(lib().gub_set_sweep(self._h, int(slots_per_cta)), "gub_set_sweep")
 
@@ -499,6 +511,34 @@ def pack_keys(keys, hits, params_idx, created_delta):
     offs[1:] = np.cumsum(lens)
     buf[b_at.value:b_at.value + len(blob)] = np.frombuffer(blob, dtype=np.uint8)
     return buf
+
+
+PROTO_OK, PROTO_TOO_LARGE, PROTO_MALFORMED = 0, 1, 2
+
+
+def proto_layout(n_msgs, msg_bytes):
+    """(offsets_at, bytes_at, total, out_bound) of gub_proto_layout."""
+    v = [C.c_size_t() for _ in range(4)]
+    _check(_entry("gub_proto_layout")(n_msgs, msg_bytes, *[C.byref(x) for x in v]), "gub_proto_layout")
+    return tuple(x.value for x in v)
+
+
+def pack_proto(messages, created_at, out=None):
+    """The one-buffer layout of gub_submit_proto_async: [int64 created_at x n][uint32 offsets x (n + 1)][message bytes].  messages: the
+    GetRateLimitsReq wire bytes of each RPC; created_at: one default per message (or one for all).  out: an array to pack into (e.g. a
+    PinnedArray's view), else a new np.uint8 array.  Returns (buffer, out_bound)."""
+    n = len(messages)
+    lens = np.fromiter((len(m) for m in messages), dtype=np.int64, count=n)
+    blob = b"".join(messages)
+    o_at, b_at, tot, bound = proto_layout(n, len(blob))
+    buf = np.zeros(tot, dtype=np.uint8) if out is None else out[:tot]
+    buf[:o_at].view(np.int64)[:] = created_at
+    offs = buf[o_at:o_at + 4 * (n + 1)].view(np.uint32)
+    offs[0] = 0
+    offs[1:] = np.cumsum(lens)
+    buf[b_at:b_at + len(blob)] = np.frombuffer(blob, dtype=np.uint8)
+    buf[b_at + len(blob):] = 0
+    return buf, bound
 
 
 def nccl_unique_id() -> bytes:

@@ -238,6 +238,28 @@ int gub_submit_keys_store_async(gub_table* t, const void* packed, size_t packed_
                                 gub_store_get_fn get, void* user,
                                 gub_resp* out, gub_store_rec* changes, uint32_t* n_changes, int* ticket);
 
+/* ---- wire bytes: V1Instance.GetRateLimits (gubernator.go:183-295) on one node, from the protobuf bytes of whole GetRateLimitsReq
+ * messages (one per RPC) to the bytes of their GetRateLimitsResp.  The device decodes every message as protobuf-go does (field numbers of
+ * gubernator.proto; unknown fields, the metadata map and known fields with another wire type skipped; open enums; created_at with
+ * presence), checks each item as gubernator.go:208-220 does (empty unique_key, then empty name: answered in-band, not evaluated;
+ * created_at absent or 0 = the message's default; behavior & 0xFF | GUB_REQ_IS_OWNER), hashes Name + "_" + UniqueKey, evaluates the
+ * call's items as one batch (message order, then item order: the host layer's aggregator) and writes each message's response as Go's
+ * proto.Marshal would: one 0x0A-framed RateLimitResp per item, zero fields omitted, the error text of gub_format_error in full.
+ * One buffer per call: [int64 created_at x n_msgs][uint32 offsets x (n_msgs + 1)][message bytes]; message m = bytes[offsets[m] ..
+ * offsets[m + 1]), offsets[0] = 0, at most 2^31 - 1 message bytes.  created_at[m] is the default of message m (gubernator.go:195 takes
+ * one epochMillis(clock.Now()) per RPC).  gub_proto_layout also returns out_bound, a safe upper bound on the output bytes. */
+enum { GUB_PROTO_OK = 0, GUB_PROTO_TOO_LARGE = 1 /* more than 1000 items: codes.OutOfRange (gubernator.go:189-193) */,
+       GUB_PROTO_MALFORMED = 2 /* what grpc-go's unmarshal rejects */ };
+int gub_proto_layout(size_t n_msgs, size_t msg_bytes, size_t* offsets_at, size_t* bytes_at, size_t* total, size_t* out_bound);
+/* After gub_wait(ticket): msg_status[m] per message, and message m's response = out_bytes[out_off[m] .. out_off[m + 1]) (empty unless
+ * GUB_PROTO_OK; nothing of a TOO_LARGE or MALFORMED message is evaluated, and the other messages are unaffected).
+ * out_bytes (out_cap >= out_bound for the call's message bytes), out_off (n_msgs + 1) and msg_status (n_msgs) must be page-locked
+ * (gub_host_alloc): the device writes them directly.  The offsets are checked on the host.  Pipelined like gub_submit_keys_async (up to
+ * gub_pipeline_depth() calls in flight, library-owned staging), except that the call returns only once its messages are decoded: the
+ * evaluation is sized by the number of items the device found. */
+int gub_submit_proto_async(gub_table* t, const void* packed, size_t packed_bytes, size_t n_msgs, const gub_clock* clk, void* out_bytes,
+                           size_t out_cap, uint64_t* out_off, uint32_t* msg_status, int* ticket);
+
 /* Page-locked host memory for request/response buffers: with these the H2D/D2H copies of gub_submit_async are truly
  * asynchronous (a Go shim allocates its batch arenas here once).  Any other host memory works too, just slower. */
 void* gub_host_alloc(size_t bytes);
