@@ -383,6 +383,22 @@ int launch_batch(gub_table* t, const gub_req* d_reqs, size_t n, const gub_clock*
   return 0;
 }
 
+void free_slot(PipeSlot& s) {
+  if (s.d_req) cudaFree(s.d_req);
+  if (s.d_resp) cudaFree(s.d_resp);
+  if (s.d_creq) cudaFree(s.d_creq);
+  if (s.d_packed) cudaFree(s.d_packed);
+  if (s.d_params) cudaFree(s.d_params);
+  if (s.in_done) cudaEventDestroy(s.in_done);
+  if (s.out_done) cudaEventDestroy(s.out_done);
+  auto& pr = s.proto;
+  void* dev[] = {pr.slot_base, pr.batch_base, pr.mcount, pr.meval, pr.mstatus, pr.msize, pr.moff, pr.items, pr.sreq, pr.keys, pr.stage};
+  for (void* p : dev) if (p) cudaFree(p);
+  if (pr.h_neval) cudaFreeHost(pr.h_neval);
+  if (pr.decoded) cudaEventDestroy(pr.decoded);
+  s = PipeSlot();
+}
+
 int ensure_slot(PipeSlot& s, size_t n) {
   if (s.cap >= n) return 0;
   if (s.d_req) cudaFree(s.d_req);
@@ -482,20 +498,7 @@ void gub_destroy(gub_table* t) {
                   t->gaux, t->gpres, t->gfrag, t->gmembers, t->ctl, t->ovf, t->trace, t->ktrace, t->inv.e};
   for (void* p : ptrs) if (p) cudaFree(p);
   free_scratch(t->scr);
-  for (auto& s : t->pipe) {
-    if (s.d_req) cudaFree(s.d_req);
-    if (s.d_resp) cudaFree(s.d_resp);
-    if (s.d_creq) cudaFree(s.d_creq);
-    if (s.d_packed) cudaFree(s.d_packed);
-    if (s.d_params) cudaFree(s.d_params);
-    if (s.in_done) cudaEventDestroy(s.in_done);
-    if (s.out_done) cudaEventDestroy(s.out_done);
-    auto& pr = s.proto;
-    void* dev[] = {pr.slot_base, pr.batch_base, pr.mcount, pr.meval, pr.mstatus, pr.msize, pr.moff, pr.items, pr.sreq, pr.keys, pr.stage};
-    for (void* p : dev) if (p) cudaFree(p);
-    if (pr.h_neval) cudaFreeHost(pr.h_neval);
-    if (pr.decoded) cudaEventDestroy(pr.decoded);
-  }
+  for (auto& s : t->pipe) free_slot(s);
   for (auto& e : t->compute_done) if (e) cudaEventDestroy(e);
   for (auto& e : t->prof_ev) cudaEventDestroy(e);
   {
@@ -992,6 +995,40 @@ int proto_ensure(PipeSlot& s, const gub::ProtoPlan& P, size_t n_msgs) {
   }
   return 0;
 }
+
+// The decode half of a wire-bytes call on `st`, after the copy of the packed buffer into s.d_packed: slot bases, decoding, batch bases
+// (the evaluable count to the mapped word) and the compaction into s.d_req; then the `decoded` event.  A.out*, A.force_global: the caller's.
+int proto_decode(PipeSlot& s, const gub::ProtoPlan& P, size_t n_msgs, gub::ProtoArgs& A, cudaStream_t st) {
+  auto& pr = s.proto;
+  A.created = reinterpret_cast<const int64_t*>(s.d_packed);
+  A.offs = reinterpret_cast<const uint32_t*>(s.d_packed + P.offsets_at);
+  A.bytes = s.d_packed + P.bytes_at;
+  A.n_msgs = (uint32_t)n_msgs;
+  A.smem = P.smem;
+  A.slot_base = pr.slot_base; A.batch_base = pr.batch_base; A.mcount = pr.mcount; A.meval = pr.meval; A.mstatus = pr.mstatus;
+  A.msize = pr.msize; A.moff = pr.moff; A.items = pr.items; A.sreq = pr.sreq; A.keys = pr.keys; A.stage = pr.stage;
+  A.reqs = s.d_req; A.resp = s.d_resp;
+  if (device_view(pr.h_neval, &A.n_eval)) return -1;
+  const unsigned grid = (unsigned)n_msgs;
+  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, st>>>(A, 0u);
+  gub::k_proto_decode<<<grid, gub::PROTO_THREADS, P.smem, st>>>(A);
+  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, st>>>(A, 1u);
+  gub::k_proto_compact<<<grid, gub::PROTO_THREADS, 0, st>>>(A);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(pr.decoded, st));
+  return 0;
+}
+
+// The encode half on `st`, once the responses of the dense batch are in A.resp: every message's bytes, offsets and status into the
+// caller's page-locked buffers.
+int proto_encode(const gub::ProtoArgs& A, cudaStream_t st) {
+  const unsigned grid = A.n_msgs;
+  gub::k_proto_encode<<<grid, gub::PROTO_THREADS, 0, st>>>(A);
+  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, st>>>(A, 2u);
+  gub::k_proto_copy_out<<<grid, gub::PROTO_THREADS, 0, st>>>(A);
+  CK(cudaGetLastError());
+  return 0;
+}
 }  // namespace
 
 extern "C" {
@@ -1038,31 +1075,13 @@ int gub_submit_proto_async(gub_table* t, const void* packed, size_t packed_bytes
   CK(cudaStreamWaitEvent(t->s_proto, s.in_done, 0));
   gub::ProtoArgs A;
   std::memset(&A, 0, sizeof A);
-  A.created = reinterpret_cast<const int64_t*>(s.d_packed);
-  A.offs = reinterpret_cast<const uint32_t*>(s.d_packed + P.offsets_at);
-  A.bytes = s.d_packed + P.bytes_at;
-  A.n_msgs = (uint32_t)n_msgs;
-  A.smem = P.smem;
-  A.slot_base = pr.slot_base; A.batch_base = pr.batch_base; A.mcount = pr.mcount; A.meval = pr.meval; A.mstatus = pr.mstatus;
-  A.msize = pr.msize; A.moff = pr.moff; A.items = pr.items; A.sreq = pr.sreq; A.keys = pr.keys; A.stage = pr.stage;
-  A.reqs = s.d_req; A.resp = s.d_resp;
-  if (device_view(pr.h_neval, &A.n_eval)) return -1;
   A.out = d_out; A.out_off = d_off; A.out_status = d_status;
-  const unsigned grid = (unsigned)n_msgs;
-  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, t->s_proto>>>(A, 0u);
-  gub::k_proto_decode<<<grid, gub::PROTO_THREADS, P.smem, t->s_proto>>>(A);
-  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, t->s_proto>>>(A, 1u);
-  gub::k_proto_compact<<<grid, gub::PROTO_THREADS, 0, t->s_proto>>>(A);
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(pr.decoded, t->s_proto));
+  if (proto_decode(s, P, n_msgs, A, t->s_proto)) return -1;
   CK(cudaEventSynchronize(pr.decoded));
   const uint32_t n_eval = *(volatile uint32_t*)pr.h_neval;
   CK(cudaStreamWaitEvent(t->s_compute, pr.decoded, 0));
   if (n_eval && launch_batch(t, s.d_req, n_eval, clk, s.d_resp, t->s_compute)) return -1;
-  gub::k_proto_encode<<<grid, gub::PROTO_THREADS, 0, t->s_compute>>>(A);
-  gub::k_proto_scan<<<1, gub::PROTO_SCAN_THREADS, 0, t->s_compute>>>(A, 2u);
-  gub::k_proto_copy_out<<<grid, gub::PROTO_THREADS, 0, t->s_compute>>>(A);
-  CK(cudaGetLastError());
+  if (proto_encode(A, t->s_compute)) return -1;
   CK(cudaEventRecord(s.out_done, t->s_compute));
   s.busy = true;
   return 0;
@@ -1653,6 +1672,11 @@ struct gub_p2p {
   // Store steps (gub_p2p_step_keys_store_local_all), allocated by the first one: [2][world][cap] inverse map of this shard's routing by
   // step parity (k_store_orig), read by the owners over peer access
   uint32_t* store_orig = nullptr;
+  // Wire-bytes steps (gub_p2p_step_proto_local_all), allocated and grown by the calls: two sets by call parity, each holding the
+  // packed copy, the decode scratch and the dense batch with its responses.  A set is reused once the call two back has been encoded.
+  PipeSlot proto_set[2];
+  uint32_t proto_calls = 0;
+  cudaStream_t s_proto = nullptr;  // decoding: waits only for its own call's copy, so it overlaps the previous call's steps
 };
 
 namespace {
@@ -1696,6 +1720,8 @@ void gub_p2p_destroy(gub_p2p* p) {
     if (r.routed) cudaEventDestroy(r.routed);
     if (r.step_done) cudaEventDestroy(r.step_done);
   }
+  for (auto& s : p->proto_set) free_slot(s);
+  if (p->s_proto) cudaStreamDestroy(p->s_proto);
   if (p->hits_q) gub_gq_destroy(p->hits_q);
   if (p->updates_q) gub_gq_destroy(p->updates_q);
   gub_nccl_comm_destroy_(p->nccl);
@@ -2356,6 +2382,118 @@ int gub_p2p_step_keys_store_local_all(gub_p2p* const* ps, uint32_t world, const 
     }
   }
   return p2p_local_all_store(ps, world, in.data(), n, clk, rs, d_out, streams);
+}
+
+}  // extern "C"
+
+namespace {
+// One shard's part in a wire-bytes call: its plan, its decode set and the arguments its kernels share.
+struct ProtoShard {
+  gub::ProtoPlan P{};
+  gub::ProtoArgs A{};
+  PipeSlot* set = nullptr;
+  size_t n_msgs = 0;
+  uint32_t n_eval = 0;
+};
+}  // namespace
+
+extern "C" {
+
+/* Wire bytes on the ring (see the header).  1. every check on every shard; 2. per shard: wait for the call two back on this parity's
+ * set, grow it; 3. per shard on its decode stream: copy, decode, compact; 4. the host waits for every decoded count; 5. S ring steps
+ * through p2p_local_all, step k ingesting [k x cap, (k + 1) x cap) of each dense batch; 6. per shard on streams[r]: encode. */
+int gub_p2p_step_proto_local_all(gub_p2p* const* ps, uint32_t world, const void* const* packed, const size_t* packed_bytes, const size_t* n_msgs,
+                                 int force_global, const gub_clock* clk, void* const* out_bytes, const size_t* out_cap, uint64_t* const* out_off,
+                                 uint32_t* const* msg_status, void* const* streams) {
+  const std::string what = "gub_p2p_step_proto_local_all";
+  if (!ps || !packed || !packed_bytes || !n_msgs || !out_bytes || !out_cap || !out_off || !msg_status || !streams || world == 0)
+    return fail(what + ": bad argument");
+  std::vector<ProtoShard> sh(world);
+  for (uint32_t r = 0; r < world; r++) {  // 1. nothing is allocated, copied or enqueued before every shard has passed
+    gub_p2p* p = ps[r];
+    ProtoShard& h = sh[r];
+    const std::string at = what + ": shard " + std::to_string(r) + ": ";
+    if (p2p_step_check(p, nullptr, 0, clk, nullptr, what.c_str())) return -1;
+    h.n_msgs = n_msgs[r];
+    if (!out_off[r] || (h.n_msgs && (!packed[r] || !out_bytes[r] || !msg_status[r]))) return fail(at + "null argument");
+    if (h.n_msgs > 0x7FFFFFFFull) return fail(at + "too many messages");
+    if (h.n_msgs) {
+      if (const char* why = gub::proto_plan(static_cast<const uint8_t*>(packed[r]), packed_bytes[r], h.n_msgs, out_cap[r], h.P)) return fail(at + why);
+    }
+    CK(cudaSetDevice(p->t->device));
+    std::memset(&h.A, 0, sizeof h.A);
+    h.A.out = h.n_msgs ? pinned_view(static_cast<uint8_t*>(out_bytes[r])) : nullptr;
+    h.A.out_off = pinned_view(reinterpret_cast<unsigned long long*>(out_off[r]));
+    h.A.out_status = h.n_msgs ? pinned_view(msg_status[r]) : nullptr;
+    if (!h.A.out_off || (h.n_msgs && (!h.A.out || !h.A.out_status)))
+      return fail(at + "out_bytes, out_off and msg_status must be page-locked host memory (gub_host_alloc)");
+    h.A.force_global = force_global ? 1u : 0u;
+  }
+  for (uint32_t r = 0; r < world; r++) {  // 2. a failed allocation fails the call before any shard routes
+    gub_p2p* p = ps[r];
+    ProtoShard& h = sh[r];
+    if (!h.n_msgs) continue;
+    CK(cudaSetDevice(p->t->device));
+    PipeSlot& s = p->proto_set[p->proto_calls & 1u];
+    if (s.busy) { CK(cudaEventSynchronize(s.out_done)); s.busy = false; }
+    if (!p->s_proto) {
+      CK(cudaStreamCreateWithFlags(&p->s_proto, cudaStreamNonBlocking));
+      CK(cudaFuncSetAttribute(gub::k_proto_decode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gub::PROTO_SMEM));
+    }
+    if (!s.out_done) CK(cudaEventCreateWithFlags(&s.out_done, cudaEventDisableTiming));
+    if (ensure_slot(s, std::max<size_t>(h.P.slots, 1)) || proto_ensure(s, h.P, h.n_msgs)) return -1;
+    const size_t need = h.P.bytes_at + h.P.msg_bytes;
+    if (s.packed_cap < need) {
+      if (s.d_packed) cudaFree(s.d_packed);
+      s.d_packed = nullptr; s.packed_cap = 0;
+      const size_t c = std::max<size_t>(need + need / 4, (size_t)1 << 20);
+      CK(cudaMalloc(&s.d_packed, c));
+      s.packed_cap = c;
+    }
+    h.set = &s;
+  }
+  for (uint32_t r = 0; r < world; r++) {  // 3. the decode of every shard
+    gub_p2p* p = ps[r];
+    ProtoShard& h = sh[r];
+    if (!h.n_msgs) continue;
+    CK(cudaSetDevice(p->t->device));
+    CK(cudaMemcpyAsync(h.set->d_packed, packed[r], h.P.bytes_at + h.P.msg_bytes, cudaMemcpyHostToDevice, p->s_proto));
+    if (proto_decode(*h.set, h.P, h.n_msgs, h.A, p->s_proto)) return -1;
+  }
+  size_t S = 0;
+  for (uint32_t r = 0; r < world; r++) {  // 4. every shard's evaluable count
+    gub_p2p* p = ps[r];
+    ProtoShard& h = sh[r];
+    if (!h.n_msgs) continue;
+    CK(cudaSetDevice(p->t->device));
+    CK(cudaEventSynchronize(h.set->proto.decoded));
+    h.n_eval = *(volatile uint32_t*)h.set->proto.h_neval;
+    S = std::max<size_t>(S, ((size_t)h.n_eval + p->cap - 1) / p->cap);
+    CK(cudaStreamWaitEvent((cudaStream_t)streams[r], h.set->proto.decoded, 0));
+  }
+  std::vector<Ingest> in(world);
+  std::vector<size_t> n(world);
+  std::vector<gub_resp*> d_out(world);
+  for (size_t k = 0; k < S; k++) {  // 5. the ring steps: exactly gub_p2p_step_local_all's on each chunk of the dense batches
+    for (uint32_t r = 0; r < world; r++) {
+      const size_t lo = k * ps[r]->cap;
+      n[r] = sh[r].n_eval > lo ? std::min<size_t>(ps[r]->cap, sh[r].n_eval - lo) : 0;
+      in[r].reqs = n[r] ? sh[r].set->d_req + lo : nullptr;
+      d_out[r] = n[r] ? sh[r].set->d_resp + lo : nullptr;
+    }
+    if (p2p_local_all(ps, world, in.data(), n.data(), clk, d_out.data(), streams)) return -1;
+  }
+  for (uint32_t r = 0; r < world; r++) {  // 6. every shard's responses, on its stream
+    gub_p2p* p = ps[r];
+    ProtoShard& h = sh[r];
+    p->proto_calls++;
+    if (!h.n_msgs) { out_off[r][0] = 0; continue; }
+    CK(cudaSetDevice(p->t->device));
+    if (proto_encode(h.A, (cudaStream_t)streams[r])) return -1;
+    CK(cudaEventRecord(h.set->out_done, (cudaStream_t)streams[r]));
+    h.set->busy = true;
+  }
+  return 0;
 }
 
 }  // extern "C"

@@ -16,6 +16,8 @@
 //                      at PROTO_OUT_FACTOR x the message's input offset (the bound needs no other message's size);
 //   k_proto_scan(2)    output offsets and statuses, straight into the caller's page-locked out_off / msg_status;
 //   k_proto_copy_out   each message's bytes from staging into the caller's page-locked out_bytes, 16 bytes per store where aligned.
+// On the ring (gub_p2p_step_proto_local_all) every shard runs the same kernels on its own RPCs; ring steps of cap items of the dense
+// batch take the place of launch_batch, and the collects fill `resp`.
 #pragma once
 #include "gub_kernels.cuh"
 
@@ -47,6 +49,7 @@ struct ProtoArgs {
   const uint8_t* bytes;      // message bytes
   uint32_t n_msgs;
   uint32_t smem;             // k_proto_decode's dynamic shared memory: messages up to this size are staged
+  uint32_t force_global;     // Behaviors.ForceGlobal (gubernator.go:232-234): every evaluable item also gets GLOBAL
   uint32_t* slot_base;       // [n_msgs + 1]
   uint32_t* batch_base;      // [n_msgs + 1]
   uint32_t *mcount, *meval, *mstatus, *msize;  // [n_msgs]: items listed, items evaluated, status, output bytes
@@ -303,7 +306,8 @@ __global__ void __launch_bounds__(PROTO_THREADS) k_proto_decode(ProtoArgs A) {
       r.hits = f.hits; r.limit = f.limit; r.duration = f.duration; r.burst = f.burst;
       r.created_at = (f.has_created && f.created_at != 0) ? f.created_at : A.created[m];  // :218-220
       r.algorithm = (uint32_t)f.algorithm;
-      r.behavior = ((uint32_t)f.behavior & 0xFFu) | GUB_REQ_IS_OWNER;  // one node: every key is ours
+      r.behavior = ((uint32_t)f.behavior & 0xFFu) | GUB_REQ_IS_OWNER | (A.force_global ? (uint32_t)GUB_BEHAVIOR_GLOBAL : 0u);  // the
+      // ring's routing clears IS_OWNER where another shard owns the key
       A.sreq[slot0 + j] = r;
       evalmask |= 1u << k;
       nev++;
@@ -354,6 +358,12 @@ struct ProtoEmit {  // d == nullptr: count only
 __device__ __noinline__ void proto_error_text(ProtoEmit& o, uint32_t code, const uint8_t* key, uint32_t key_len, int32_t algorithm) {
   if (code == GUB_ERR_UNIQUE_KEY_EMPTY) { o.s("field 'unique_key' cannot be empty"); return; }
   if (code == GUB_ERR_NAMESPACE_EMPTY) { o.s("field 'namespace' cannot be empty"); return; }
+  if (code == GUB_ERR_PEER_TIMEOUT) {  // gubernator.go:374 wrapping the deadline error of a peer call that timed out (ring steps only)
+    o.s("Error while fetching rate limit '");
+    for (uint32_t q = 0; q < key_len; q++) o.c(key[q]);
+    o.s("' from peer: context deadline exceeded");
+    return;
+  }
   if (code < GUB_ERR_INVALID_ALGORITHM || code > GUB_ERR_TABLE_FULL) return;
   o.s("Error while apply rate limit for '");
   for (uint32_t q = 0; q < key_len; q++) o.c(key[q]);

@@ -47,6 +47,9 @@ void gub_format_error(int err_code, const char* key, int32_t algorithm, char* ou
                     algo_scope(algorithm));
       break;
     case GUB_ERR_TABLE_FULL: std::snprintf(out, cap, "%srate limit table is full", head); break;
+    case GUB_ERR_PEER_TIMEOUT:  // gubernator.go:374 wrapping the deadline error of a timed-out peer call
+      std::snprintf(out, cap, "Error while fetching rate limit '%s' from peer: context deadline exceeded", key);
+      break;
     default: if (cap) out[0] = 0;
   }
 }

@@ -55,7 +55,8 @@ EXPORTS = ["gub_create", "gub_destroy", "gub_last_error", "gub_abi_version", "gu
            "gub_p2p_connect_local", "gub_p2p_step", "gub_p2p_step_streams", "gub_p2p_status", "gub_p2p_enable_global", "gub_nccl_unique_id",
            "gub_p2p_nccl_init", "gub_p2p_nccl_init_local", "gub_global_tick", "gub_gq_dropped", "gub_set_sweep", "gub_set_trace", "gub_get_trace", "gub_get_trace_raw", "gub_get_ktrace", "gub_keys_layout", "gub_submit_keys_async", "gub_global_tick_local_all", "gub_p2p_step_local_all",
            "gub_p2p_step_keys", "gub_p2p_step_keys_local_all", "gub_p2p_step_mixed_local_all",
-           "gub_submit_keys_store_async", "gub_p2p_step_keys_store_local_all", "gub_proto_layout", "gub_submit_proto_async"]
+           "gub_submit_keys_store_async", "gub_p2p_step_keys_store_local_all", "gub_proto_layout", "gub_submit_proto_async",
+           "gub_p2p_step_proto_local_all"]
 
 
 class Config(C.Structure):
@@ -159,6 +160,7 @@ _LATE_ARGTYPES = {
     "gub_p2p_step_keys_store_local_all": [_pvp, C.c_uint32, _pvp, _psz, _psz, _vp, _sz, C.c_int64, _vp, STORE_GET_FN, _vp, _pvp, _pvp, _pvp, _pvp],
     "gub_proto_layout": [_sz, _sz, _psz, _psz, _psz, _psz],
     "gub_submit_proto_async": [_vp, _vp, _sz, _sz, _vp, _vp, _sz, _vp, _vp, C.POINTER(C.c_int)],
+    "gub_p2p_step_proto_local_all": [_pvp, C.c_uint32, _pvp, _psz, _psz, C.c_int, _vp, _pvp, _psz, _pvp, _pvp, _pvp],
 }
 
 
@@ -567,6 +569,19 @@ def p2p_step_keys_local_all(p2ps, packed_ptrs, packed_bytes, ns, params, created
     _check(_entry("gub_p2p_step_keys_local_all")((C.c_void_p * W)(*[p._h for p in p2ps]), W, (C.c_void_p * W)(*packed_ptrs), (C.c_size_t * W)(*packed_bytes),
                                              (C.c_size_t * W)(*ns), params.ctypes.data if len(params) else None, len(params), int(created_base),
                                              clk.ctypes.data, (C.c_void_p * W)(*out_ptrs), (C.c_void_p * W)(*streams)), "gub_p2p_step_keys_local_all")
+
+
+def p2p_step_proto_local_all(p2ps, packed_ptrs, packed_bytes, n_msgs, clk, out_ptrs, out_caps, out_off_ptrs, status_ptrs, streams,
+                             force_global=False):
+    """GetRateLimitsReq wire bytes on every shard of this process (gub_p2p_step_proto_local_all): packed_ptrs[r] = shard r's pack_proto()
+    buffer (host memory), n_msgs[r] its message count.  out_ptrs[r] (out_caps[r] bytes, at least pack_proto's bound), out_off_ptrs[r]
+    (n_msgs[r] + 1 uint64) and status_ptrs[r] (n_msgs[r] uint32) must be page-locked (PinnedArray): shard r's responses, valid once
+    streams[r] has completed the call.  force_global: Behaviors.ForceGlobal."""
+    W = len(p2ps)
+    _check(_entry("gub_p2p_step_proto_local_all")((C.c_void_p * W)(*[p._h for p in p2ps]), W, (C.c_void_p * W)(*packed_ptrs),
+                                              (C.c_size_t * W)(*packed_bytes), (C.c_size_t * W)(*n_msgs), 1 if force_global else 0, clk.ctypes.data,
+                                              (C.c_void_p * W)(*out_ptrs), (C.c_size_t * W)(*out_caps), (C.c_void_p * W)(*out_off_ptrs),
+                                              (C.c_void_p * W)(*status_ptrs), (C.c_void_p * W)(*streams)), "gub_p2p_step_proto_local_all")
 
 
 def p2p_step_mixed_local_all(p2ps, req_ptrs, packed_ptrs, packed_bytes, ns, params, created_base, clk, out_ptrs, streams):

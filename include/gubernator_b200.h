@@ -458,6 +458,29 @@ int gub_p2p_step_keys_store_local_all(gub_p2p* const* ps, uint32_t world, const 
                                       const size_t* n, const gub_params* params, size_t n_params, int64_t created_base,
                                       const gub_clock* clk, gub_store_get_fn get, void* user, gub_resp* const* d_out,
                                       gub_store_rec* const* changes, uint32_t* const* n_changes, void* const* streams);
+/* gub_submit_proto_async on the ring of this process: shard r takes the GetRateLimitsReq messages of packed[r] (host memory in the
+ * layout of gub_proto_layout; any split of the RPCs over the shards is valid) and writes their responses to its own page-locked
+ * out_bytes[r] (out_cap[r] >= out_bound) / out_off[r] (n_msgs[r] + 1) / msg_status[r] (n_msgs[r]), valid once streams[r] has completed
+ * the call (no tickets: the ring's convention).  Per item the rules of gub_submit_proto_async apply unchanged (decoding, the checks of
+ * gubernator.go:208-220, created_at per message, behavior & 0xFF | GUB_REQ_IS_OWNER, TOO_LARGE and MALFORMED messages evaluate nothing).
+ *   force_global   Behaviors.ForceGlobal (gubernator.go:232-234): every item that passes the checks also gets GUB_BEHAVIOR_GLOBAL.
+ *   evaluation     n_r = the evaluable items of shard r (message order, then item order), S = max_r ceil(n_r / cap): the call performs
+ *                  S steps, and in step k shard r ingests its items [k x cap, min(n_r, (k + 1) x cap)) as the records of exactly the step
+ *                  gub_p2p_step_local_all would perform.  For each key, items apply in (step, source rank, source index) order; with a
+ *                  contiguous split and every n_r <= cap that is message order, and the bytes equal those of gub_submit_proto_async on one
+ *                  table for the concatenated messages.  S = 0: no step, no epoch advances, the responses are still written.
+ *   GLOBAL rings   as for record steps: a GLOBAL item another shard owns is answered from the replica and its hits are queued.
+ *   timeouts       an item whose owner never answered (GUB_ERR_PEER_TIMEOUT) gets the error text of gubernator.go:374, "Error while
+ *                  fetching rate limit '<key>' from peer: context deadline exceeded".
+ * Blocks until every shard's messages are decoded (the steps are sized by the items the devices found) and, on each shard, until the
+ * call two back is encoded: two sets of library-owned scratch per shard alternate by call parity, so consecutive calls need no
+ * synchronisation by the caller and a call's decode overlaps the previous call's steps.  The sets grow with the input (allocating
+ * synchronises the device).  Refused (text in gub_last_error()) before anything is copied or enqueued on any shard, so no epoch advances:
+ * offsets that fail the checks of gub_submit_proto_async, out_cap below the bound, outputs outside page-locked memory, a shard that fails
+ * the checks of gub_p2p_step_local_all, more than 2^31 - 1 messages on a shard; a failed allocation fails the call before any shard routes. */
+int gub_p2p_step_proto_local_all(gub_p2p* const* ps, uint32_t world, const void* const* packed, const size_t* packed_bytes, const size_t* n_msgs,
+                                 int force_global, const gub_clock* clk, void* const* out_bytes, const size_t* out_cap, uint64_t* const* out_off,
+                                 uint32_t* const* msg_status, void* const* streams);
 /* Device-side waits are bounded (a dead peer must not hang the GPU); a wait that gave up marks the step: *error_out != 0 and the
  * call fails with text in gub_last_error().  Requests whose owner never answered carry GUB_ERR_PEER_TIMEOUT in-band.  Costs a
  * device synchronisation: poll at your own cadence. */
